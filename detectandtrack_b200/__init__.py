@@ -1,4 +1,4 @@
-"""detectandtrack_b200 — B200 (sm_100a) hot path behind the DetectAndTrack
+"""detectandtrack_b200 — H100 (sm_90a) hot path behind the DetectAndTrack
 cfg / model-builder / tools surface.  Host code is Python mirroring the
 reference's module names (core/, modeling/, ops/, utils/); the arithmetic runs in
 hand-written CUDA through the C ABI in include/dt_b200.h (``_lib``).  There is

@@ -146,7 +146,7 @@ def call(name, *args):
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise RuntimeError('detectandtrack_b200 needs a CUDA device (B200, sm_100a); '
+        raise RuntimeError('detectandtrack_b200 needs a CUDA device (H100, sm_90a); '
                            'there is no CPU fallback.')
     return torch
 

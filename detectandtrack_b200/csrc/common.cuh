@@ -1,4 +1,4 @@
-// Shared helpers for the DetectAndTrack B200 C-ABI library (sm_100a only).
+// Shared helpers for the DetectAndTrack C-ABI library (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -48,6 +48,14 @@ static inline cudaError_t grant_dyn_smem(K kernel, int bytes, DynSmemGrant* g) {
 }
 
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
+
+// SM count of the current device (grid sizing of persistent / split-K launches); 132 on an H100 SXM
+static inline int num_sms() {
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1)
+    return 132;
+  return sms;
+}
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 }  // namespace dt

@@ -1,4 +1,4 @@
-// Conv3d / Conv2d / FC as ONE implicit-GEMM kernel on the 5th-gen tensor cores (tcgen05),
+// Conv3d / Conv2d / FC as ONE implicit-GEMM kernel on the Hopper tensor cores (wgmma),
 // NDHWC activations, fused AffineChannel (+bias) + residual / top-down-upsample add + ReLU.
 //
 // Replaces, on the reference's hot path:
@@ -11,18 +11,19 @@
 //
 // GEMM view: D[m, n] = sum_{tap, c} A[m @ tap, c] * W[tap, n, c]
 //   m = output position (img, t, ho, wo) tiled as TH x TW spatial patches (TH*TW <= 128 rows)
-//   n = output channel, BLOCK_N in {32, 64, 128, 256};  k-block = one tap x 128 bytes of channels
+//   n = output channel, BLOCK_N in {32, 64, 128};  k-block = one tap x 128 bytes of channels
 //   A tile: one 5-D TMA box (C=128B, TW, TH, 1, 1) at the tap-shifted coordinate; out-of-bounds
 //           elements (spatial / temporal zero padding, ragged edge tiles, channel tail) are
 //           zero-filled by the TMA unit, so padding costs no instructions and no branches.
 //   W tile: 3-D TMA box (C=128B, BLOCK_N, 1) of the pre-packed [tap][Cout][Cin] weights.
-//   Both land in the 128B-swizzled K-major layout tcgen05.mma reads directly.
-// Roles (640 threads, 1 CTA / SM, persistent over tiles):
-//   warp 0, 19: TMA producers (activation / weight tiles; one elected lane each)   smem ring: full[]/empty[]
-//   warp 1    : TMEM allocator + MMA issuer (one lane)   tcgen05.mma -> TMEM, tcgen05.commit
+//   Both land in the 128B-swizzled K-major layout wgmma reads directly.
+// Roles (384 threads = 3 warpgroups, 1 CTA / SM, persistent over tiles):
+//   warp 0, 1 : TMA producers (activation / weight tiles; one elected lane each)   smem ring: full[]/empty[]
 //   warp 2    : TMA store warp                           staged output chunks -> global, recycles staging slots
-//   warps 3-18: epilogue; TMEM -> registers (tcgen05.ld), scale/bias/residual/ReLU in fp32, staged in
-//               128B-swizzled smem chunks.  Two TMEM accumulator stages overlap it with the next tile's MMAs.
+//   warp 3    : idle (pads the producer warpgroup)
+//   warps 4-11: two consumer warpgroups, rows 0-63 and 64-127 of the tile: wgmma into register accumulators
+//               (64 x BLOCK_N each), then the epilogue: scale/bias/residual/ReLU in fp32, staged in 128B-swizzled
+//               smem chunks.  The producers run ahead into the next tile's k-blocks while the epilogue runs.
 // Everything is handed over through mbarriers; there is no block-wide barrier inside the tile loop.
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -86,9 +87,9 @@ struct ConvKernelParams {
   int nrbuf;                   // > 0: bf16 residual chunks arrive by TMA in a ring of this many staged chunks
   int res_up;                  // with nrbuf > 0: the residual is the (Ho/2, Wo/2) map of the FPN top-down add;
                                // its (TH/2 x TW/2) box is loaded and every row is read by its four children
-  int ab_format;               // tcgen05 kind::f16 operand format: 1 bf16, 0 fp16 (kind::tf32: 2)
-  int round_tf32;              // fp32 output is rounded (RNE) to tf32 so the next tcgen05 kind::tf32 MMA,
-                               // which TRUNCATES its 32-bit operands, sees exactly representable values
+  int ab_format;               // 16-bit operand format: 1 bf16, 0 fp16 (TF32 kernels ignore it)
+  int round_tf32;              // fp32 output is rounded (RNE) to tf32 so the next tf32 MMA, which ignores the
+                               // low mantissa bits of its 32-bit operands, sees exactly representable values
 };
 
 __device__ __forceinline__ float round_to_tf32(float v) {
@@ -97,10 +98,10 @@ __device__ __forceinline__ float round_to_tf32(float v) {
   return __uint_as_float(u & 0xFFFFE000u);
 }
 
-constexpr int EPI_WARPS = 16;                         // 4 TMEM lane groups x 4 column quarters
-constexpr int EPI_THREADS = EPI_WARPS * 32;
-constexpr int CONV_THREADS = 128 + EPI_THREADS;       // + two TMA producer warps, the MMA issuer and the TMA store warp
-constexpr int B_WARP = 3 + EPI_WARPS;                 // weight-tile producer (warps 3 .. 3+EPI_WARPS-1 are the epilogue)
+constexpr int EPI_WARPS = 8;                          // two consumer warpgroups
+constexpr int CONV_THREADS = 128 + EPI_WARPS * 32;    // + the producer warpgroup (two TMA producer warps, the TMA store warp)
+constexpr int B_WARP = 1;                             // weight-tile producer
+constexpr int EPI_WARP0 = 4;                          // first consumer warp
 
 template <int BN>
 struct ConvCfg {
@@ -108,9 +109,8 @@ struct ConvCfg {
   static constexpr int B_BYTES = BN * 128;
   static constexpr int KB_BYTES = A_BYTES + B_BYTES;   // one k-block of both operands
   static constexpr int MAX_STAGES = 8;
-  static constexpr int TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;
   static constexpr int C_BYTES = 128 * 128;            // one staged output chunk: 128 rows x 128 B
-  static constexpr int BAR_BYTES = 384;                // mbarriers + TMEM base pointer
+  static constexpr int BAR_BYTES = 384;                // mbarriers
   static constexpr int FIXED_BYTES = BAR_BYTES;
   static constexpr int BUDGET = 227 * 1024;
   // K-heavy layers want a deep operand ring; K-light (HBM-bound) layers want output staging buffers so the
@@ -118,7 +118,7 @@ struct ConvCfg {
   static int tab_bytes(int kiters) { return ((kiters + 2) * 24 + 127) / 128 * 128; }   // k-block schedule
   static void split(int kiters, bool res_tma, bool split_out, bool out_f32, int* stages, int* ks, int* ncbuf, int* nrbuf) {
     const int chunks = BN / (out_f32 ? 32 : 64);        // staged chunks per tile
-    int c = (kiters >= 12 && !split_out) ? ((BN >= 256) ? 1 : 2) : 4;   // split (hi, lo) output: two slots of two buffers
+    int c = (kiters >= 12 && !split_out) ? 2 : 4;       // split (hi, lo) output: two slots of two buffers
     if (!split_out && c > 2 * chunks) c = chunks >= 1 ? 2 * chunks : 2;   // two tiles of staging are enough
     const int r = res_tma ? ((kiters >= 12 || split_out) ? 2 : 4) : 0;      // split output: a residual slot is a chunk pair
     const int rb = split_out ? 2 * r : r;
@@ -146,25 +146,17 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvKernelParams& p, int 
   return c;
 }
 
-#ifdef DT_CONV_TRACE
-__device__ long long g_conv_trace[64 * 16];
-#define TRACE(ti, k) do { if (blockIdx.x == 0 && (ti) < 64) g_conv_trace[(ti) * 16 + (k)] = clock64(); } while (0)
-#define TRACE_ADD(ti, k, v) do { if (blockIdx.x == 0 && (ti) < 64) g_conv_trace[(ti) * 16 + (k)] += (v); } while (0)
-#else
-#define TRACE(ti, k) do {} while (0)
-#define TRACE_ADD(ti, k, v) do {} while (0)
-#endif
-
 // SPLIT: the output (and the residual) rows are [hi | lo] pairs (the x3 modes' intermediate activations); a template
-// parameter so that the plain kernels do not carry the pair logic's registers (the epilogue sits at the 96-register cap).
-template <int BN, bool TF32, bool SPLIT>
+// parameter so that the plain kernels do not carry the pair logic's registers.
+// KIND: MMA operand type, 0 bf16, 1 fp16, 2 tf32 (wgmma.cuh).
+template <int BN, int KIND, bool SPLIT>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
                const ConvKernelParams p) {
   using Cfg = ConvCfg<BN>;
   const int STAGES = p.nstages;
-  constexpr int BK = TF32 ? 32 : 64;                 // elements per 128-byte k-block
+  constexpr int BK = KIND == 2 ? 32 : 64;            // elements per 128-byte k-block
   // SWIZZLE_128B operands need 1024-byte aligned tiles: the dynamic window is declared with that alignment
   // (no static shared memory in this kernel) and checked once below instead of spending a kilobyte on slack
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -174,13 +166,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* bars = reinterpret_cast<uint64_t*>(rbuf + p.nrbuf * rslot_bytes);
   uint64_t* full = bars;                       // [STAGES]  operands landed
   uint64_t* empty = bars + STAGES;             // [STAGES]  operands consumed by the MMAs
-  uint64_t* tmem_full = bars + 2 * STAGES;     // [2]       accumulator complete
-  uint64_t* tmem_empty = tmem_full + 2;        // [2]       accumulator read out
-  uint64_t* r_full = tmem_full + 4;            // [4]       residual chunk landed
-  uint64_t* r_empty = tmem_full + 8;           // [4]       residual chunk consumed
-  uint64_t* c_full = tmem_full + 12;           // [4]       output chunk staged by all epilogue warps
-  uint64_t* c_free = tmem_full + 16;           // [4]       staging slot read out by its TMA store
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_full + 20);
+  uint64_t* r_full = bars + 2 * STAGES;        // [4]       residual chunk landed
+  uint64_t* r_empty = r_full + 4;              // [4]       residual chunk consumed
+  uint64_t* c_full = r_full + 8;               // [4]       output chunk staged by all epilogue warps
+  uint64_t* c_free = r_full + 12;              // [4]       staging slot read out by its TMA store
   // k-block schedule of one tile: what the producers add to the tile's base coordinates for k-block j.
   // Built once; walking taps / channel chunks with carry logic in the producer loop costs more cycles per
   // k-block than a narrow tile's MMAs take.
@@ -220,23 +209,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     prefetch_tmap(&tmB);
     prefetch_tmap(&tmC);
     if (p.nrbuf > 0) prefetch_tmap(&tmR);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 2); mbar_init(&empty[s], 1); }    // full: A and B producers
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], EPI_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 2); mbar_init(&empty[s], EPI_WARPS); }  // full: A and B producers
     for (int s = 0; s < 4; ++s) {
       mbar_init(&r_full[s], 1); mbar_init(&r_empty[s], EPI_WARPS);
       mbar_init(&c_full[s], EPI_WARPS); mbar_init(&c_free[s], 1);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_base_smem);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation, tensor-map prefetch, the k-block
-  // schedule) touched only kernel parameters and shared memory, so it may overlap the tail of the previous kernel of
-  // the stream; no global data is read or written before this wait.  The trigger lets the NEXT kernel's prologue do
-  // the same under this one's tail (its CTAs become resident as this kernel's CTAs retire: 1 CTA / SM by shared memory).
+  // Programmatic dependent launch: everything above (barrier init, tensor-map prefetch, the k-block schedule) touched
+  // only kernel parameters and shared memory, so it may overlap the tail of the previous kernel of the stream; no
+  // global data is read or written before this wait.  The trigger lets the NEXT kernel's prologue do the same under
+  // this one's tail (its CTAs become resident as this kernel's CTAs retire: 1 CTA / SM by shared memory).
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
@@ -246,11 +230,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 0 || warp == B_WARP) {
     // ===================== TMA producers =====================
     // Two warps: warp 0 loads the activation tiles (and the residual ring), warp B_WARP the weight tiles; both
-    // arm the same full[] barrier with their own byte count.  One warp doing both spends ~500 cycles per
-    // k-block on scalar bookkeeping + TMA issue, more than a 128-column tile's MMAs take (256 cycles).
-    // The whole warp runs the loop (warp-uniform control flow and addresses, so descriptors / coordinates
-    // stay in uniform registers); one elected lane issues.  A divergent `if (lane == 0)` around the loop
-    // makes the compiler wrap every UTMALDG / UTCHMMA in an elect-broadcast "waterfall" loop.
+    // arm the same full[] barrier with their own byte count, so the scalar bookkeeping of the two operands runs
+    // in parallel.  The whole warp runs the loop (warp-uniform control flow and addresses, so descriptors /
+    // coordinates stay in uniform registers); one elected lane issues.
     const bool load_b = warp != 0;
     int stage = 0; uint32_t phase = 0;
     int rslot = 0; uint32_t rphase = 0;
@@ -266,10 +248,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int h_base = tc.thi * p.TH * p.sH - p.pH;
       const int t_base = p.row_planes ? 0 : (tc.tti * p.TT + p.t_first) * p.sT - p.pT;
       const int n_base = tc.nt * BN;
-#ifdef DT_CONV_TRACE
-      long long acc_wait = 0, acc_issue = 0;
-#endif
-      if (lane == 0 && !load_b) TRACE(tile / gridDim.x, 0);
       for (int ki = 0; ki < kiters; ki += KS) {
         const int nk = min(KS, kiters - ki);
         // this stage's k-blocks from the schedule (uniform loads), then ONE elected issue block
@@ -284,14 +262,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             x0[q] = e.x; x1[q] = w_base + e.y; x2[q] = h_base + e.z; x3[q] = t_base + e.w;
           }
         }
-#ifdef DT_CONV_TRACE
-        const long long tw0 = clock64();
-#endif
         mbar_wait_u(empty_u + stage * 8, phase ^ 1);
-#ifdef DT_CONV_TRACE
-        acc_wait += clock64() - tw0;
-        const long long tw2 = clock64();
-#endif
         if (elect_one()) {
           const uint32_t bar = full_u + stage * 8;
           const uint32_t dst = smem_u + stage * stage_bytes;
@@ -304,15 +275,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             if (nk > 1) tma_load_5d_u(dst + Cfg::KB_BYTES, &tmA, bar, x0[1], x1[1], x2[1], x3[1], n);
           }
         }
-#ifdef DT_CONV_TRACE
-        acc_issue += clock64() - tw2;
-#endif
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      if (lane == 0 && !load_b) TRACE(tile / gridDim.x, 1);
-#ifdef DT_CONV_TRACE
-      if (lane == 0 && !load_b) { TRACE_ADD(tile / gridDim.x, 10, acc_wait); TRACE_ADD(tile / gridDim.x, 12, acc_issue); }
-#endif
       if (p.nrbuf > 0 && !load_b) {
         // residual chunks of this tile (bf16, same box as the output chunks), consumed in order by the epilogue
         const int ncols = min(BN, p.Cout - n_base);
@@ -331,54 +295,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           if (++rslot == p.nrbuf) { rslot = 0; rphase ^= 1; }
         }
       }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp, one elected lane issues) =====================
-    const uint32_t idesc = make_idesc(128, BN, TF32 ? 2 : p.ab_format);
-    const uint32_t smem_u = smem_u32(smem);
-    const uint32_t full_u = smem_u32(full);
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const int KS = p.ks;
-    const uint32_t stage_bytes = (uint32_t)KS * Cfg::KB_BYTES;
-    int stage = 0; uint32_t phase = 0;
-    int as = 0; uint32_t aphase = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      mbar_wait(&tmem_empty[as], aphase ^ 1);
-      tcgen05_fence_after();
-      const uint32_t d_tmem = tmem_u + as * BN;
-      if (lane == 0) TRACE(tile / gridDim.x, 2);
-#ifdef DT_CONV_TRACE
-      long long acc_wf = 0;
-#endif
-      for (int ki = 0; ki < kiters; ki += KS) {
-        const int nk = min(KS, kiters - ki);
-#ifdef DT_CONV_TRACE
-        const long long tw1 = clock64();
-#endif
-        mbar_wait_u(full_u + stage * 8, phase);
-#ifdef DT_CONV_TRACE
-        acc_wf += clock64() - tw1;
-#endif
-        tcgen05_fence_after();
-        const uint32_t a_addr = smem_u + stage * stage_bytes;
-        if (elect_one()) {
-          for (int q = 0; q < nk; ++q) {
-            const uint64_t adesc = make_sw128_kmajor_desc(a_addr + q * Cfg::KB_BYTES);
-            const uint64_t bdesc = make_sw128_kmajor_desc(a_addr + q * Cfg::KB_BYTES + Cfg::A_BYTES);
-#pragma unroll
-            for (int k = 0; k < 4; ++k)          // 4 x 32 B = one 128-byte swizzle row of K
-              umma<TF32>(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (ki | q | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);            // frees the smem slot when these MMAs retire
-          if (ki + nk >= kiters) umma_commit(&tmem_full[as]);   // accumulator ready for the epilogue
-        }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (lane == 0) TRACE(tile / gridDim.x, 3);
-#ifdef DT_CONV_TRACE
-      if (lane == 0) TRACE_ADD(tile / gridDim.x, 11, acc_wf);
-#endif
-      if (++as == 2) { as = 0; aphase ^= 1; }
     }
   } else if (warp == 2) {
     // ===================== TMA store warp =====================
@@ -419,241 +335,198 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
     if (elect_one()) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  } else {
-    // ===================== epilogue (warps 3..18) =====================
-    // TMEM -> registers -> fp32 epilogue -> 128B-swizzled smem chunk -> TMA store (store warp).
-    // Sixteen warps (four per scheduler): warp w reads TMEM lane group (w & 3) and owns column quarter
-    // ((w - 3) >> 2) of every staged 128-byte row (32 bytes: 16 bf16 or 8 fp32 outputs).  No block-wide
-    // barriers: staging slots are handed over through mbarriers (c_full / c_free), scale / bias are uniform
-    // 16-byte loads through L1, ReLU rides on the bf16 pack (cvt.rn.relu), the TMEM load of chunk c+1 is issued
-    // as soon as chunk c's accumulators have been consumed, and the accumulator is released to the MMA warp
-    // right after its last column has been read.  The TMA store writes whole 128-byte lines and clips rows /
-    // channels outside the tensor, so ragged tiles need no predication on the store side.
-    const int lg = warp & 3;                   // TMEM lane group this warp may access
-    const int part = (warp - 3) >> 2;          // which 32-byte quarter of the staged row this warp fills
-    const int row = lg * 32 + lane;            // accumulator row == TMEM lane == staging row
-    int rr = row;
-    const int tw = rr % p.TW; rr /= p.TW;
-    const int th = rr % p.TH; rr /= p.TH;
-    const int tl = rr % p.TT;
-    const int nl = rr / p.TT;                  // >= TB for the unused tail rows of a short tile
+  } else if (warp >= EPI_WARP0) {
+    // ===================== consumers (warps 4..11): wgmma, then the epilogue =====================
+    // Warpgroup g computes rows 64g .. 64g+63 of the tile.  Thread (warp q of its group, lane l) holds the accumulators
+    // of rows 16q + l/4 and 16q + l/4 + 8 of that half, columns 8j + 2(l%4) + {0, 1} (wgmma.cuh).  The epilogue turns
+    // each (row, column pair) into one 4-byte (bf16) / 8-byte (fp32) store into a 128B-swizzled staging chunk (the
+    // eight rows of a warp hit eight different 16-byte units: conflict-free), which the store warp writes out by TMA.
+    // The TMA store writes whole 128-byte lines and clips rows / channels outside the tensor, so ragged tiles need
+    // no predication on the store side.
+    const int wg = (warp - EPI_WARP0) >> 2;
+    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: row0 and row0 + 8
+    const int cq = lane & 3;
     const bool out_f32 = p.out_f32 != 0;
     constexpr bool split_out = SPLIT;
     const bool relu = p.relu != 0;
     const int res_mode = p.res_mode;
     const int Cout = p.Cout;
-    const int CW = out_f32 ? 32 : 64;          // output columns per 128-byte staged row
-    const int colw = out_f32 ? 8 : 16;         // columns this warp owns per chunk
+    const int JPC = out_f32 ? 4 : 8;           // 8-column accumulator groups per 128-byte staged chunk
     const int nslots = split_out ? p.ncbuf / 2 : p.ncbuf;
     const uint32_t slot_bytes = split_out ? 2u * Cfg::C_BYTES : (uint32_t)Cfg::C_BYTES;
     const uint32_t cbuf_u32 = smem_u32(cbuf);
     const uint32_t rbuf_u32 = smem_u32(rbuf);
     const bool res_tma = p.nrbuf > 0;
     const bool res_ldg = res_mode != 0 && !res_tma;
-    // residual row of this thread inside a ring slot: its own row, or (top-down add) the row of its parent
-    // position in the (TH/2 x TW/2) box of the coarser map
-    const int rrow = p.res_up ? ((nl * p.TT + tl) * (p.TH >> 1) + (th >> 1)) * (p.TW >> 1) + (tw >> 1) : row;
-    const uint32_t rrow_smem = (uint32_t)rrow * 128u;
-    const uint32_t rswz = (uint32_t)(rrow & 7);
-    const uint32_t rq0 = (((uint32_t)(2 * part)) ^ rswz) << 4, rq1 = (((uint32_t)(2 * part + 1)) ^ rswz) << 4;
-    int rslot = 0; uint32_t rphase = 0;
-    const uint32_t row_smem = (uint32_t)row * 128u;
-    const uint32_t swz = (uint32_t)(row & 7);
-    const uint32_t q0 = (((uint32_t)(2 * part)) ^ swz) << 4, q1 = (((uint32_t)(2 * part + 1)) ^ swz) << 4;
+    // per row i: position inside the tile, staging row offset and swizzle, residual ring row (top-down add: the row of
+    // its parent position in the (TH/2 x TW/2) box of the coarser map)
+    int tw_[2], th_[2], tl_[2], nl_[2];
+    uint32_t srow[2], sswz[2], rrow[2], rswz[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      int rr = row0 + 8 * i;
+      srow[i] = (uint32_t)rr * 128u; sswz[i] = (uint32_t)(rr & 7);
+      tw_[i] = rr % p.TW; rr /= p.TW;
+      th_[i] = rr % p.TH; rr /= p.TH;
+      tl_[i] = rr % p.TT;
+      nl_[i] = rr / p.TT;                      // >= TB for the unused tail rows of a short tile
+      const int rp = p.res_up ? ((nl_[i] * p.TT + tl_[i]) * (p.TH >> 1) + (th_[i] >> 1)) * (p.TW >> 1) + (tw_[i] >> 1)
+                              : row0 + 8 * i;
+      rrow[i] = (uint32_t)rp * 128u; rswz[i] = (uint32_t)(rp & 7);
+    }
     const float* __restrict__ g_scale = p.scale;
     const float* __restrict__ g_bias = p.bias;
-    int as = 0; uint32_t aphase = 0;
+    const uint32_t smem_u = smem_u32(smem) + (uint32_t)wg * (64u * 128u);   // this warpgroup's 64 rows of the A tile
+    const uint32_t full_u = smem_u32(full);
+    const int KS = p.ks;
+    const uint32_t stage_bytes = (uint32_t)KS * Cfg::KB_BYTES;
+    int stage = 0; uint32_t phase = 0;
+    int rslot = 0; uint32_t rphase = 0;
     int slot = 0; uint32_t sphase = 0;
+    float acc[BN / 2];
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const TileCoord tc = decode_tile(p, tile);
-      bool valid = true;
-      size_t rpos = 0;
-      if (res_ldg) {                           // per-thread residual row (fp32 / upsample-add paths only)
-        const int ho = tc.thi * p.TH + th, wo = tc.twi * p.TW + tw;
-        const int t = tc.tti * p.TT + tl, n = tc.tbi * p.TB + nl;
-        valid = (nl < p.TB) && (ho < p.Ho) && (wo < p.Wo) && (t < p.To) && (n < p.N);
-        rpos = (res_mode == 2) ? ((size_t)(n * p.To + t) * (p.Ho >> 1) + (ho >> 1)) * (p.Wo >> 1) + (wo >> 1)
-                               : ((size_t)(n * p.To + t) * p.Ho + ho) * p.Wo + wo;
+      // ---- main loop: one wgmma group per k-block; a ring stage goes back to the producers once the group of the
+      // NEXT stage's last k-block is issued and the stage's own groups retired (one stage stays in flight).  The
+      // wgmmas sit outside any branch so that they are not serialized.
+      int prev = -1;
+      for (int ki = 0; ki < kiters; ++ki) {
+        const int q = KS == 2 ? (ki & 1) : 0;          // k-block inside the ring stage
+        if (q == 0) mbar_wait_u(full_u + stage * 8, phase);
+        const uint32_t off = stage * stage_bytes + q * Cfg::KB_BYTES;
+        const uint64_t adesc = make_sw128_desc(smem_u + off);
+        const uint64_t bdesc = make_sw128_desc(smem_u32(smem) + off + Cfg::A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)                    // 4 x 32 B = one 128-byte swizzle row of K
+          wgmma<BN, KIND>(acc, adesc + 2 * k, bdesc + 2 * k, (ki | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        if (q == KS - 1 || ki == kiters - 1) {
+          if (q == 1) wgmma_wait<2>(); else wgmma_wait<1>();   // only this stage's q + 1 groups may still run
+          if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+          prev = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+
+      // ---- epilogue
+      bool valid[2] = {true, true};
+      size_t rpos[2] = {0, 0};
+      if (res_ldg) {                           // per-thread residual rows (fp32 / upsample-add paths only)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int ho = tc.thi * p.TH + th_[i], wo = tc.twi * p.TW + tw_[i];
+          const int t = tc.tti * p.TT + tl_[i], n = tc.tbi * p.TB + nl_[i];
+          valid[i] = (nl_[i] < p.TB) && (ho < p.Ho) && (wo < p.Wo) && (t < p.To) && (n < p.N);
+          rpos[i] = (res_mode == 2) ? ((size_t)(n * p.To + t) * (p.Ho >> 1) + (ho >> 1)) * (p.Wo >> 1) + (wo >> 1)
+                                    : ((size_t)(n * p.To + t) * p.Ho + ho) * p.Wo + wo;
+        }
       }
       const int nbase = tc.nt * BN;
       const int ncols = min(BN, Cout - nbase);     // live output columns of this tile
-      if (threadIdx.x == 96) TRACE(tile / gridDim.x, 4);
-
-      mbar_wait(&tmem_full[as], aphase);
-      if (threadIdx.x == 96) TRACE(tile / gridDim.x, 5);
-      tcgen05_fence_after();
-      const uint32_t taddr = tmem_base + as * BN + ((uint32_t)(lg * 32) << 16) + (uint32_t)(colw * part);
-      uint32_t r[16];
-      if (out_f32) tmem_ld_32x32b_x8_lo(taddr, r); else tmem_ld_32x32b_x16(taddr, r);
-#pragma unroll 1
-      for (int cc = 0; cc < ncols; cc += CW) {
-        const int c0 = cc + colw * part;           // first column (inside the tile) this warp handles
-        const int cbase = nbase + c0;
-        const bool more = cc + CW < ncols;
-        // AffineChannel scale / bias of this warp's columns: uniform 16-byte loads (L1 hits after first touch)
-        float sc[16], bi[16];
-        if (cbase + colw <= Cout) {
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            if (q < (colw >> 2)) {
-              const float4 s4 = g_scale ? __ldg(reinterpret_cast<const float4*>(g_scale + cbase) + q) : make_float4(1.f, 1.f, 1.f, 1.f);
-              const float4 b4 = g_bias ? __ldg(reinterpret_cast<const float4*>(g_bias + cbase) + q) : make_float4(0.f, 0.f, 0.f, 0.f);
-              sc[4 * q] = s4.x; sc[4 * q + 1] = s4.y; sc[4 * q + 2] = s4.z; sc[4 * q + 3] = s4.w;
-              bi[4 * q] = b4.x; bi[4 * q + 1] = b4.y; bi[4 * q + 2] = b4.z; bi[4 * q + 3] = b4.w;
+      for (int j = 0; j < BN / 8; ++j) {
+        if (8 * j >= ncols) break;
+        const int jc = j % JPC;                    // 8-column group inside the staged chunk
+        const int col = nbase + 8 * j + 2 * cq;    // first of this thread's two output channels
+        if (jc == 0) {
+          // chunk start: the staging slot must have been read out by the TMA store that used it last (c_free), and
+          // the producer's residual chunk must have landed
+          mbar_wait(&c_free[slot], sphase ^ 1);
+          if (res_tma) mbar_wait(&r_full[rslot], rphase);
+        }
+        float sc0 = 1.f, sc1 = 1.f, bi0 = 0.f, bi1 = 0.f;
+        if (col + 2 <= Cout) {
+          if (g_scale) { const float2 s2 = __ldg(reinterpret_cast<const float2*>(g_scale + col)); sc0 = s2.x; sc1 = s2.y; }
+          if (g_bias) { const float2 b2 = __ldg(reinterpret_cast<const float2*>(g_bias + col)); bi0 = b2.x; bi1 = b2.y; }
+        } else if (col < Cout) {                   // ragged channel tail
+          if (g_scale) sc0 = __ldg(g_scale + col);
+          if (g_bias) bi0 = __ldg(g_bias + col);
+        }
+        const uint32_t dst_slot = cbuf_u32 + (uint32_t)slot * slot_bytes;
+        const uint32_t src_slot = rbuf_u32 + (uint32_t)rslot * rslot_bytes;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float v0 = fmaf(acc[4 * j + 2 * i], sc0, bi0);
+          float v1 = fmaf(acc[4 * j + 2 * i + 1], sc1, bi1);
+          if (out_f32) {
+            if (res_mode != 0 && valid[i]) {
+              const float* rp = reinterpret_cast<const float*>(p.residual) + rpos[i] * p.res_ld + col;
+              if (col + 2 <= Cout) {
+                const float2 q = __ldg(reinterpret_cast<const float2*>(rp));
+                v0 += q.x; v1 += q.y;
+                if (split_out) {                                     // residual = hi + lo
+                  const float2 ql = __ldg(reinterpret_cast<const float2*>(rp + p.res_lo_off));
+                  v0 += ql.x; v1 += ql.y;
+                }
+              } else if (col < Cout) {
+                v0 += __ldg(rp) + (split_out ? __ldg(rp + p.res_lo_off) : 0.f);
+              }
             }
-          }
-        } else {                                   // ragged channel tail
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const bool in = j < colw && cbase + j < Cout;
-            sc[j] = (in && g_scale) ? __ldg(g_scale + cbase + j) : 1.f;
-            bi[j] = (in && g_bias) ? __ldg(g_bias + cbase + j) : 0.f;
+            if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            // 8 bytes at chunk column 8 jc + 2 cq: 16-byte unit 2 jc + cq / 2, offset 8 (cq & 1)
+            const uint32_t off = ((((uint32_t)(2 * jc + (cq >> 1))) ^ sswz[i]) << 4) + 8u * (cq & 1);
+            const uint32_t dst = dst_slot + srow[i] + off;
+            if (split_out) {
+              const float h0 = round_to_tf32(v0), h1 = round_to_tf32(v1);
+              sts_f2(dst + Cfg::C_BYTES, round_to_tf32(v0 - h0), round_to_tf32(v1 - h1));   // lo: the slot's second buffer
+              v0 = h0; v1 = h1;
+            } else if (p.round_tf32) {
+              v0 = round_to_tf32(v0); v1 = round_to_tf32(v1);
+            }
+            sts_f2(dst, v0, v1);
+          } else {
+            // 4 bytes at chunk column 8 jc + 2 cq: 16-byte unit jc, offset 4 cq
+            if (res_tma) {
+              const uint32_t src = src_slot + rrow[i] + ((((uint32_t)jc) ^ rswz[i]) << 4) + 4u * cq;
+              uint32_t r2 = lds_b1(src);
+              v0 += __uint_as_float(r2 << 16); v1 += __uint_as_float(r2 & 0xffff0000u);
+              if (SPLIT) { r2 = lds_b1(src + Cfg::C_BYTES); v0 += __uint_as_float(r2 << 16); v1 += __uint_as_float(r2 & 0xffff0000u); }
+            } else if (res_ldg && valid[i]) {
+              const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.residual) + rpos[i] * p.res_ld + col;
+              if (col + 2 <= Cout) {
+                uint32_t r2 = __ldg(reinterpret_cast<const unsigned int*>(rp));
+                v0 += __uint_as_float(r2 << 16); v1 += __uint_as_float(r2 & 0xffff0000u);
+                if (SPLIT) {                                          // residual = hi + lo (bf16 pairs)
+                  r2 = __ldg(reinterpret_cast<const unsigned int*>(rp + p.res_lo_off));
+                  v0 += __uint_as_float(r2 << 16); v1 += __uint_as_float(r2 & 0xffff0000u);
+                }
+              } else if (col < Cout) {
+                v0 += __bfloat162float(rp[0]) + (SPLIT ? __bfloat162float(rp[p.res_lo_off]) : 0.f);
+              }
+            }
+            const uint32_t dst = dst_slot + srow[i] + ((((uint32_t)jc) ^ sswz[i]) << 4) + 4u * cq;
+            if (split_out) {
+              // bf16 pair storage: hi = bf16(v), lo = bf16(v - hi) (v - hi is exact in fp32); hi + lo carries 16
+              // mantissa bits, which three bf16 MMAs per k-block turn into an fp32-accurate product
+              if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+              const uint32_t h = pack_bf16x2(v0, v1);
+              sts_b1(dst + Cfg::C_BYTES, pack_bf16x2(v0 - __uint_as_float(h << 16), v1 - __uint_as_float(h & 0xffff0000u)));
+              sts_b1(dst, h);
+            } else {
+              sts_b1(dst, relu ? pack_bf16x2_relu(v0, v1) : pack_bf16x2(v0, v1));
+            }
           }
         }
-        float v[16];
-        if (out_f32) {
-          // ---- fp32 output: this warp owns 8 columns = 32 bytes
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] = fmaf(__uint_as_float(r[j]), sc[j], bi[j]);
-          if (more) {
-            tmem_ld_32x32b_x8_lo(taddr + cc + CW, r);
-          } else {                                 // accumulator fully read: release it to the MMA warp
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[as]);
-          }
-          if (res_mode != 0 && valid) {
-            const float* rp = reinterpret_cast<const float*>(p.residual) + rpos * p.res_ld + cbase;
-            if (cbase + 8 <= Cout) {
-#pragma unroll
-              for (int j = 0; j < 8; j += 4) {
-                const float4 q = __ldg(reinterpret_cast<const float4*>(rp + j));
-                v[j] += q.x; v[j + 1] += q.y; v[j + 2] += q.z; v[j + 3] += q.w;
-                if (split_out) {                                     // residual = hi + lo
-                  const float4 ql = __ldg(reinterpret_cast<const float4*>(rp + p.res_lo_off + j));
-                  v[j] += ql.x; v[j + 1] += ql.y; v[j + 2] += ql.z; v[j + 3] += ql.w;
-                }
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                if (cbase + j < Cout) v[j] += __ldg(rp + j) + (split_out ? __ldg(rp + p.res_lo_off + j) : 0.f);
-            }
-          }
-          if (relu) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.f);
-          }
-        } else {
-          // ---- bf16 output: this warp owns 16 columns = 32 bytes
-          // residual rows first: the global loads overlap the TMEM wait
-          uint4 resq[2];
-          const bool res_on = res_ldg && valid;
-          const bool res_vec = res_on && (cbase + 16 <= Cout);
-          const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.residual) + rpos * p.res_ld + cbase;
-          if (res_vec) {
-            resq[0] = __ldg(reinterpret_cast<const uint4*>(rp));
-            resq[1] = __ldg(reinterpret_cast<const uint4*>(rp + 8));
-          }
-          // the producer warp prefetched this chunk's residual rows (zero-filled outside the tensor) into the swizzled ring
-          if (res_tma) mbar_wait(&r_full[rslot], rphase);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaf(__uint_as_float(r[j]), sc[j], bi[j]);
-          if (more) {
-            tmem_ld_32x32b_x16(taddr + cc + CW, r);
-          } else {                                 // accumulator fully read: release it to the MMA warp
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[as]);
-          }
-          auto add16 = [&](const uint4& a, const uint4& b) {          // 16 bf16 residual values onto v
-            const uint32_t w8[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              v[2 * e] += __uint_as_float(w8[e] << 16);
-              v[2 * e + 1] += __uint_as_float(w8[e] & 0xffff0000u);
-            }
-          };
+        if (jc == JPC - 1 || 8 * (j + 1) >= ncols) {
+          // chunk complete: hand the residual slot back, then generic-proxy smem writes -> visible to the async
+          // proxy, then this warp's arrival on the staging slot
           if (res_tma) {
-            // read this thread's 32 bytes (hi, then the lo chunk in the slot's second buffer), then hand the slot back
-            const uint32_t src = rbuf_u32 + (uint32_t)rslot * rslot_bytes + rrow_smem;
-            add16(lds_u4(src + rq0), lds_u4(src + rq1));
-            if (SPLIT) add16(lds_u4(src + Cfg::C_BYTES + rq0), lds_u4(src + Cfg::C_BYTES + rq1));
             __syncwarp();
             if (lane == 0) mbar_arrive(&r_empty[rslot]);
             if (++rslot == p.nrbuf) { rslot = 0; rphase ^= 1; }
-          } else if (res_vec) {
-            add16(resq[0], resq[1]);
-            if (SPLIT)                                                // residual = hi + lo (bf16 pairs)
-              add16(__ldg(reinterpret_cast<const uint4*>(rp + p.res_lo_off)), __ldg(reinterpret_cast<const uint4*>(rp + p.res_lo_off + 8)));
-          } else if (res_on) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (cbase + j < Cout) v[j] += __bfloat162float(rp[j]) + (SPLIT ? __bfloat162float(rp[p.res_lo_off + j]) : 0.f);
           }
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&c_full[slot]);
+          if (++slot == nslots) { slot = 0; sphase ^= 1; }
         }
-
-        // staging slot: the TMA store that used it last must have read it out (c_free)
-        mbar_wait(&c_free[slot], sphase ^ 1);
-        if (threadIdx.x == 96) TRACE(tile / gridDim.x, 6);
-        const uint32_t dst = cbuf_u32 + (uint32_t)slot * slot_bytes + row_smem;
-        if (out_f32) {
-          if (split_out) {
-            float lo[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { const float hi = round_to_tf32(v[j]); lo[j] = round_to_tf32(v[j] - hi); v[j] = hi; }
-            const uint32_t dst_lo = dst + Cfg::C_BYTES;               // the lo chunk uses the slot's second buffer
-            sts_f4(dst_lo + q0, lo[0], lo[1], lo[2], lo[3]);
-            sts_f4(dst_lo + q1, lo[4], lo[5], lo[6], lo[7]);
-          } else if (p.round_tf32) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = round_to_tf32(v[j]);
-          }
-          sts_f4(dst + q0, v[0], v[1], v[2], v[3]);
-          sts_f4(dst + q1, v[4], v[5], v[6], v[7]);
-        } else {
-          uint32_t h[8];
-          if (split_out) {
-            // bf16 pair storage: hi = bf16(v), lo = bf16(v - hi) (v - hi is exact in fp32); hi + lo carries 16
-            // mantissa bits, which three bf16 MMAs per k-block turn into an fp32-accurate product
-            uint32_t l[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float a = v[2 * j], b = v[2 * j + 1];
-              if (relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
-              h[j] = pack_bf16x2(a, b);
-              l[j] = pack_bf16x2(a - __uint_as_float(h[j] << 16), b - __uint_as_float(h[j] & 0xffff0000u));
-            }
-            const uint32_t dst_lo = dst + Cfg::C_BYTES;
-            sts_b4(dst_lo + q0, l[0], l[1], l[2], l[3]);
-            sts_b4(dst_lo + q1, l[4], l[5], l[6], l[7]);
-          } else if (relu) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) h[j] = pack_bf16x2_relu(v[2 * j], v[2 * j + 1]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) h[j] = pack_bf16x2(v[2 * j], v[2 * j + 1]);
-          }
-          sts_b4(dst + q0, h[0], h[1], h[2], h[3]);
-          sts_b4(dst + q1, h[4], h[5], h[6], h[7]);
-        }
-        // generic-proxy smem writes -> visible to the async proxy, then this warp's arrival on the slot
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&c_full[slot]);
-        if (threadIdx.x == 96) TRACE(tile / gridDim.x, 7);
-        if (++slot == nslots) { slot = 0; sphase ^= 1; }
       }
-      if (threadIdx.x == 96) TRACE(tile / gridDim.x, 9);
-      if (++as == 2) { as = 0; aphase ^= 1; }
     }
   }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
 }
 
 // ------------------------------------------------------------------ host side (encode_map: tc_common.cuh)
@@ -698,12 +571,12 @@ static int encode_out_map(CUtensorMap* m, void* y, int out_f32, int Cout, int Wo
   return encode_map(m, out_f32 != 0 ? 1 : 0, 5, y, d, st, b, e);
 }
 
-template <int BN, bool TF32, bool SPLIT>
+template <int BN, int KIND, bool SPLIT>
 static int launch_conv1(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
                        const ConvKernelParams& p, int grid, cudaStream_t stream) {
   using Cfg = ConvCfg<BN>;
   static DynSmemGrant grant;
-  DT_CHECK_CUDA(grant_dyn_smem(conv_tc_kernel<BN, TF32, SPLIT>, Cfg::BUDGET, &grant));
+  DT_CHECK_CUDA(grant_dyn_smem(conv_tc_kernel<BN, KIND, SPLIT>, Cfg::BUDGET, &grant));
   ConvKernelParams q = p;
   const int kiters = p.kT * p.kH * p.kW * p.kchunks * p.nsub;
   DT_CHECK_ARG(kiters <= 2048, "conv: %d k-blocks per tile exceed the schedule table", kiters);
@@ -712,9 +585,8 @@ static int launch_conv1(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
   const int smem = Cfg::smem_bytes(kiters, q.nstages, q.ks, q.ncbuf, q.nrbuf, p.split_out != 0);
   DT_CHECK_ARG(q.nstages >= 2 && smem <= Cfg::BUDGET, "conv: smem split failed (%d stages, %d B)", q.nstages, smem);
   // DT_PDL=1 in the environment launches with programmatic stream serialization (the kernel waits on griddepcontrol
-  // before its first global access).  Measured on B200 (profiles/r02_pdl_ab.md): no gain inside the captured step
-  // (126.0 vs 126.3 clips/s bf16x3, 329.6 vs 330.4 bf16) — the replayed graph has no launch gaps left to hide — so plain
-  // stream order stays the default.
+  // before its first global access).  Plain stream order is the default: inside the captured CUDA graph of a step
+  // there are no launch gaps left for it to hide.
   static const bool pdl = [] { const char* e = getenv("DT_PDL"); return e && e[0] == '1'; }();
   cudaLaunchConfig_t lc;
   memset(&lc, 0, sizeof(lc));
@@ -723,23 +595,27 @@ static int launch_conv1(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = at; lc.numAttrs = pdl ? 1 : 0;
-  DT_CHECK_CUDA(cudaLaunchKernelEx(&lc, conv_tc_kernel<BN, TF32, SPLIT>, tmA, tmB, tmC, tmR, q));
+  DT_CHECK_CUDA(cudaLaunchKernelEx(&lc, conv_tc_kernel<BN, KIND, SPLIT>, tmA, tmB, tmC, tmR, q));
   return 0;
 }
 
-template <int BN, bool TF32>
-static int launch_conv(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
+template <int BN, int KIND>
+static int launch_conv2(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
+                        const ConvKernelParams& p, int grid, cudaStream_t stream) {
+  return p.split_out ? launch_conv1<BN, KIND, true>(tmA, tmB, tmC, tmR, p, grid, stream)
+                     : launch_conv1<BN, KIND, false>(tmA, tmB, tmC, tmR, p, grid, stream);
+}
+
+// operand kind from the descriptor: tf32, else ab_format (1 bf16, 0 fp16)
+template <int BN>
+static int launch_conv(bool tf32, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
                        const ConvKernelParams& p, int grid, cudaStream_t stream) {
-  return p.split_out ? launch_conv1<BN, TF32, true>(tmA, tmB, tmC, tmR, p, grid, stream)
-                     : launch_conv1<BN, TF32, false>(tmA, tmB, tmC, tmR, p, grid, stream);
+  if (tf32) return launch_conv2<BN, 2>(tmA, tmB, tmC, tmR, p, grid, stream);
+  return p.ab_format == 0 ? launch_conv2<BN, 1>(tmA, tmB, tmC, tmR, p, grid, stream)
+                          : launch_conv2<BN, 0>(tmA, tmB, tmC, tmR, p, grid, stream);
 }
 
 }  // namespace dt
-
-#ifdef DT_CONV_TRACE
-extern "C" int dt_conv_trace_write(const long long* in) { return cudaMemcpyToSymbol(dt::g_conv_trace, in, sizeof(long long) * 64 * 16) != cudaSuccess; }
-extern "C" int dt_conv_trace_read(long long* out) { return cudaMemcpyFromSymbol(out, dt::g_conv_trace, sizeof(long long) * 64 * 16) != cudaSuccess; }
-#endif
 
 using namespace dt;
 
@@ -815,17 +691,16 @@ extern "C" int dt_conv3d(const dt_conv_desc* d, const void* x, const void* w, co
   DT_CHECK_ARG(!p.split_in || (p.a_lo_off + d->Cin <= in_ld && p.b_lo_off >= d->Cin), "dt_conv3d: x3 lo halves do not fit the rows");
   DT_CHECK_ARG(!p.split_out || p.out_lo_off + d->Cout <= out_ld, "dt_conv3d: x3 output lo half does not fit the row");
 
-  int BN = d->Cout >= 256 ? 256 : (d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : 32));
-  if (d->Cout > 128 && d->Cout < 256) BN = 128;
+  // each consumer warpgroup keeps a 64 x BN fp32 accumulator in registers: BN / 2 per thread, so 128 is the widest
+  // column tile that leaves the epilogue room under the 168-register cap of a 384-thread CTA
+  const int BN = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : 32);
   // bf16 same-shape residual: its chunks are prefetched by TMA into a shared-memory ring (coalesced 128-byte
-  // rows instead of one 32-byte global load per thread).  The ring needs room, so these layers use 128-wide
-  // column tiles (they are the K-light 1x1 expansions of the bottlenecks: HBM-bound, not MMA-bound).
+  // rows instead of 4-byte global loads per thread pair).
   // The FPN top-down add (res_mode 2) goes the same way when the tile is even-sized (tile origins are then even
   // too): the (TH/2 x TW/2) box of the coarser map is loaded and each row serves its four children.
   const bool res_even = (TH % 2 == 0) && (TW % 2 == 0);
   const bool res_tma = (d->res_mode == 1 || (d->res_mode == 2 && res_even)) && !out_f32 && !tf32 &&
                        ((uintptr_t)residual % 16) == 0;
-  if (res_tma && BN > 128) BN = 128;
   p.t_first = d->out_t_count > 0 ? d->out_t_first : 0;
   p.nrbuf = res_tma ? 1 : 0;                         // ring depth is chosen with the smem split at launch
   p.res_up = (res_tma && d->res_mode == 2) ? 1 : 0;
@@ -874,14 +749,13 @@ extern "C" int dt_conv3d(const dt_conv_desc* d, const void* x, const void* w, co
   } else {
     tmR = tmC;
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   DT_CHECK_CUDA(cudaGetDevice(&dev));
   DT_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
 #define DT_LAUNCH(BNv)                                                                      \
-  return tf32 ? launch_conv<BNv, true>(tmA, tmB, tmC, tmR, p, grid, stream) : launch_conv<BNv, false>(tmA, tmB, tmC, tmR, p, grid, stream)
+  return launch_conv<BNv>(tf32, tmA, tmB, tmC, tmR, p, grid, stream)
   switch (BN) {
-    case 256: DT_LAUNCH(256);
     case 128: DT_LAUNCH(128);
     case 64: DT_LAUNCH(64);
     default: DT_LAUNCH(32);
@@ -915,11 +789,9 @@ extern "C" int dt_conv_plan(const dt_conv_desc* d, int residual_aligned, dt_conv
   const bool pointwise = d->kT == 1 && d->kH == 1 && d->kW == 1 && d->pT == 0 && d->pH == 0 && d->pW == 0;
   const TileShape ts = pick_tile(Ho, Wo, To, d->N, pointwise ? 256 : 256 / d->sW, pointwise ? 256 : 256 / d->sH,
                                  pointwise || d->sT == 1);
-  int BN = d->Cout >= 256 ? 256 : (d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : 32));
-  if (d->Cout > 128 && d->Cout < 256) BN = 128;
+  const int BN = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : 32);
   const bool res_even = (ts.th % 2 == 0) && (ts.tw % 2 == 0);
   const bool res_tma = (d->res_mode == 1 || (d->res_mode == 2 && res_even)) && !d->out_f32 && !tf32 && residual_aligned;
-  if (res_tma && BN > 128) BN = 128;
   const bool split_in = (d->x3 & 1) != 0, split_out = (d->x3 & 2) != 0;
   memset(o, 0, sizeof(*o));
   o->BN = BN; o->TH = ts.th; o->TW = ts.tw; o->TT = ts.tt; o->TB = ts.tb;
@@ -928,7 +800,6 @@ extern "C" int dt_conv_plan(const dt_conv_desc* d, int residual_aligned, dt_conv
   o->tiles = (int)(mt * cdiv(d->Cout, BN));
   o->useful_rows = (double)Ho * Wo * To * d->N / ((double)mt * 128.0);
   switch (BN) {
-    case 256: plan_split<256>(o->kiters, res_tma, split_out, d->out_f32 != 0, o); break;
     case 128: plan_split<128>(o->kiters, res_tma, split_out, d->out_f32 != 0, o); break;
     case 64: plan_split<64>(o->kiters, res_tma, split_out, d->out_f32 != 0, o); break;
     default: plan_split<32>(o->kiters, res_tma, split_out, d->out_f32 != 0, o); break;
@@ -1009,9 +880,9 @@ extern "C" int dt_conv1_7x7s2(const void* x_padded, int F, int Hp, int Wp, int C
   }
   CUtensorMap tmC;
   if (encode_out_map(&tmC, y, out_f32, x3 ? out_ld : Cout, Wo, Ho, 1, F, out_ld, ts)) return 1;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   DT_CHECK_CUDA(cudaGetDevice(&dev));
   DT_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
-  return tf32 ? launch_conv<64, true>(tmA, tmB, tmC, tmC, p, grid, stream) : launch_conv<64, false>(tmA, tmB, tmC, tmC, p, grid, stream);
+  return launch_conv<64>(tf32, tmA, tmB, tmC, tmC, p, grid, stream);
 }

@@ -650,7 +650,7 @@ using namespace dt;
 
 static int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
-  const long long cap = 148ll * 16;
+  const long long cap = num_sms() * 16ll;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 

@@ -1,10 +1,11 @@
-// sm_100a building blocks: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma /
-// commit / ld) and the UMMA shared-memory / instruction descriptors.  Inline PTX only.
+// sm_90a building blocks: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / commit / wait, wgmma.cuh) and the
+// wgmma shared-memory matrix descriptor.  Inline PTX only.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace dt {
 namespace tc {
@@ -115,80 +116,13 @@ __device__ __forceinline__ void tma_load_5d_u(uint32_t dst, const CUtensorMap* m
       : "memory");
 }
 
-// ----------------------------------------------------------------- tcgen05 --
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {    // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]   (kind::f16: fp16/bf16 inputs; kind::tf32: 32-bit inputs)
-template <bool TF32>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (TF32) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i = TMEM lane base+i)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// same load into the low half of a 32-register array (lets one array serve both epilogue layouts)
-__device__ __forceinline__ void tmem_ld_32x32b_x16_lo(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
+// ------------------------------------------------------------------- wgmma --
+// fence before the first wgmma of a batch (orders earlier register / shared-memory accesses of the accumulators),
+// commit the batch as one group, wait until at most N groups of this warpgroup are still in flight
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // ------------------------------------------------- shared-memory vector access / packing --
 __device__ __forceinline__ float4 lds_f4(uint32_t addr) {
@@ -206,6 +140,17 @@ __device__ __forceinline__ void sts_f4(uint32_t addr, float a, float b, float c,
 }
 __device__ __forceinline__ void sts_b4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ uint32_t lds_b1(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ void sts_f2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void sts_b1(uint32_t addr, uint32_t a) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
 }
 // {lo, hi} fp32 -> packed bf16x2 (round to nearest even); the relu form clamps negatives to +0 in the same op
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
@@ -228,36 +173,19 @@ __device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, uint32_t src_
                : "memory");
 }
 
-__device__ __forceinline__ void tmem_ld_32x32b_x8_lo(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory matrix descriptor, K-major operand, 128-byte swizzle:
-//   rows are 128 B apart, 8-row groups 1024 B apart (SBO), LBO unused for swizzled K-major,
-//   bits 46-47 = descriptor version 1 (sm_100), bits 61-63 = 2 (SWIZZLE_128B).
-// The tile base must be 1024-byte aligned; stepping along K inside the 128-byte row is done by
-// adding (bytes >> 4) to the low word (the swizzle is a function of the absolute smem address).
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
+// wgmma shared-memory matrix descriptor, 128-byte swizzle:
+//   bits 0-13 start address >> 4, 16-29 leading byte offset >> 4, 32-45 stride byte offset >> 4, 62-63 layout (1 = SWIZZLE_128B).
+// K-major operand: rows are 128 B apart, 8-row groups 1024 B apart (SBO), LBO unused.  MN-major operand read one
+// 64-element swizzle atom wide along M / N: only the 1024-byte stride between 8-row groups along K is used, and it is
+// written to both offset fields.  The tile base must be 1024-byte aligned; stepping along K inside the 128-byte row is
+// done by adding (bytes >> 4) to the low word (the swizzle is a function of the absolute smem address).
+__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, bool mn_major = false) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address   bits [0,14)
-  d |= (uint64_t)1 << 16;                             // LBO (ignored)   bits [16,30)
+  d |= (uint64_t)(mn_major ? 1024 >> 4 : 1) << 16;    // LBO             bits [16,30)
   d |= (uint64_t)(1024 >> 4) << 32;                   // SBO = 1024 B    bits [32,46)
-  d |= (uint64_t)1 << 46;                             // version         bits [46,48)
-  d |= (uint64_t)2 << 61;                             // SWIZZLE_128B    bits [61,64)
+  d |= (uint64_t)1 << 62;                             // SWIZZLE_128B    bits [62,64)
   return d;
-}
-
-// UMMA instruction descriptor: fp32 accumulate, A and B K-major, dense.
-//   bits 4-5 D format (1 = f32); 7-9 A format; 10-12 B format (kind::f16: 0 = f16, 1 = bf16;
-//   kind::tf32: 2 = tf32); bit 15/16 A/B major (0 = K); 17-22 N>>3; 24-28 M>>4.
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int ab_format) {
-  return (1u << 4) | ((uint32_t)ab_format << 7) | ((uint32_t)ab_format << 10) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
 }
 
 }  // namespace tc

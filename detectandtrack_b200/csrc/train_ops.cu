@@ -1,11 +1,11 @@
 // Training-step kernels of the data-parallel path (BASELINE.json configs[4]; the reference builds these with
 // model.AddGradientOperators + add_parameter_update_ops, lib/modeling/model_builder.py:908-985):
 //
-//   dt_wgrad            Conv / ConvNd filter gradient on the tcgen05 tensor cores:
+//   dt_wgrad            Conv / ConvNd filter gradient on the tensor cores (wgmma):
 //                         dW[tap][co][ci] = sum over positions of gz[pos, co] * x[pos @ tap, ci]
 //                       a GEMM whose K axis is the position axis.  Both operands are read from CHANNEL-MAJOR PLANES
 //                       ([N, T, C, plane], plane = the zero-bordered (H+2p) x (W+2p) map flattened), so a position run is
-//                       contiguous (a K-major operand for tcgen05, staged by TMA with the 128B swizzle) and a filter ROW
+//                       contiguous (a K-major operand for wgmma, staged by TMA with the 128B swizzle) and a filter ROW
 //                       offset (kh) is a constant offset along the flattened plane (rows are padded to a multiple of 8
 //                       positions, so the offset keeps TMA's 16-byte alignment of the innermost coordinate; the physical
 //                       zero border supplies the padding, TMA's out-of-bounds zero fill the plane ends and the temporal
@@ -43,8 +43,28 @@ struct WgradParams {
   float* dW;              // [taps][Cout][Cin] fp32, accumulated into (caller zeroes)
 };
 
-constexpr int WG_THREADS = 192;       // warp 0 TMA producer, warp 1 TMEM + MMA issuer, warps 2-5 epilogue
+constexpr int WG_THREADS = 384;       // warp 0 TMA producer (warps 1-3 idle), warps 4-11 two consumer warpgroups
+constexpr int WG_CONSUMER_WARPS = 8;
 constexpr int WG_STAGES = 4;
+
+// Consumers of both wgrad kernels: warpgroup g accumulates rows (output channels) 64g .. 64g+63 of the 128-row tile in
+// registers (fragment layout: wgmma.cuh) and adds them into dW with red.global.  Cin is even, so a thread's column pair
+// is either wholly inside the filter or wholly outside.
+template <int NB>
+__device__ __forceinline__ void wgrad_red(const float (&acc)[NB], float* dW, int Cout, int Cin, int tap, int row_base, int col_base) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < NB / 4; ++j) {
+    const int col = col_base + 8 * j + 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int row = row_base + ((warp - 4) >> 2) * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+      if (row < Cout && col < Cin)
+        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dW + ((size_t)tap * Cout + row) * Cin + col),
+                     "f"(acc[4 * j + 2 * i]), "f"(acc[4 * j + 2 * i + 1]) : "memory");
+    }
+  }
+}
 
 template <int BN>
 __global__ void __launch_bounds__(WG_THREADS, 1)
@@ -53,21 +73,14 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * ST_BYTES);
   uint64_t* empty = full + WG_STAGES;
-  uint64_t* acc_full = empty + WG_STAGES;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(acc_full + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();
     prefetch_tmap(&tmG); prefetch_tmap(&tmX);
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(acc_full, 1);
+    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], WG_CONSUMER_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<(BN < 32 ? 32 : BN)>(tmem_base_smem);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
 
   // work item: (tap, m tile, n tile, k split)
   int w = blockIdx.x;
@@ -80,7 +93,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
                                                  // aligned TMA coordinate); the column offset selects the pre-shifted copy kw
   const int dt_ = kt - p.pT;
   // k-blocks = (image, frame, chunk) triples; frames whose tap-shifted source frame is outside the clip contribute zero
-  // (temporal zero padding) and are skipped by producer and issuer alike
+  // (temporal zero padding) and are skipped by producer and consumers alike
   const long long total = (long long)p.N * p.T * p.kchunks;
   const long long k0 = total * ks / p.ksplit, k1 = total * (ks + 1) / p.ksplit;
 
@@ -107,77 +120,41 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
       }
       if (++chunk == p.kchunks) { chunk = 0; if (++t == p.T) { t = 0; ++n; } }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc(128, BN, 1);
+  } else if (warp >= 4) {
+    const uint32_t a_base = smem_u32(smem) + (uint32_t)((warp - 4) >> 2) * (64u * 128u);   // this warpgroup's 64 rows
     int stage = 0; uint32_t phase = 0;
     long long r = k0 / p.kchunks;
     int chunk = (int)(k0 - r * p.kchunks);
     int t = (int)(r % p.T);
+    long long kb = k0;
+    // walk to the next live k-block (the wgmmas below then sit in the loop body, not under a branch)
+    auto skip_dead = [&]() {
+      while (kb < k1 && (t + dt_ < 0 || t + dt_ >= p.T)) { ++kb; if (++chunk == p.kchunks) { chunk = 0; if (++t == p.T) t = 0; } }
+    };
+    skip_dead();
+    const bool any = kb < k1;          // a range made only of temporally padded frames accumulates nothing
+    float acc[BN / 2];
+    int prev = -1;
     uint32_t first = 1;
-    for (long long kb = k0; kb < k1; ++kb) {
-      const int ts = t + dt_;
-      if (ts >= 0 && ts < p.T) {
-        mbar_wait(&full[stage], phase);
-        tcgen05_fence_after();
-        const uint32_t a_addr = smem_u32(smem) + stage * ST_BYTES;
-        if (elect_one()) {
-          const uint64_t adesc = make_sw128_kmajor_desc(a_addr);
-          const uint64_t bdesc = make_sw128_kmajor_desc(a_addr + A_BYTES);
+    while (kb < k1) {
+      mbar_wait(&full[stage], phase);
+      const uint64_t adesc = make_sw128_desc(a_base + stage * ST_BYTES);
+      const uint64_t bdesc = make_sw128_desc(smem_u32(smem) + stage * ST_BYTES + A_BYTES);
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma<false>(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, (first && k == 0) ? 0u : 1u);
-          umma_commit(&empty[stage]);
-        }
-        first = 0;
-        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (++chunk == p.kchunks) { chunk = 0; if (++t == p.T) t = 0; }
+      for (int k = 0; k < 4; ++k) wgmma<BN, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (first && k == 0) ? 0u : 1u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+      prev = stage;
+      first = 0;
+      if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+      ++kb; if (++chunk == p.kchunks) { chunk = 0; if (++t == p.T) t = 0; }
+      skip_dead();
     }
-    if (elect_one()) umma_commit(acc_full);          // fires when every MMA above has retired (immediately if none)
-  } else {
-    // epilogue warps 2..5: TMEM lane group (warp & 3), 32 rows each.  While the MMAs run these warps are idle, so they
-    // replay the k-block walk to learn whether this CTA accumulated anything at all (a range made only of temporally
-    // padded frames leaves the accumulator unwritten).
-    bool nothing = true;
-    {
-      long long r = k0 / p.kchunks;
-      int chunk = (int)(k0 - r * p.kchunks);
-      int t = (int)(r % p.T);
-      for (long long kb = k0; kb < k1 && nothing; ) {
-        const int ts = t + dt_;
-        if (ts >= 0 && ts < p.T) nothing = false;
-        const long long step = p.kchunks - chunk;           // jump to the next frame
-        kb += step; chunk = 0; if (++t == p.T) t = 0;
-      }
-    }
-    mbar_wait(acc_full, 0);
-    tcgen05_fence_after();
-    const int lg = warp & 3;
-    const int row = mt * 128 + lg * 32 + lane;
-    if (!nothing) {
-      float* out = p.dW + ((size_t)tap * p.Cout + row) * p.Cin + nt * BN;
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        uint32_t r[16];
-        tmem_ld_32x32b_x16(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)c0, r);
-        tmem_ld_wait();
-        if (row < p.Cout) {
-          const int col = nt * BN + c0;
-          if (col + 16 <= p.Cin && (p.Cin & 3) == 0) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(out + c0 + 4 * q), "f"(__uint_as_float(r[4 * q])),
-                           "f"(__uint_as_float(r[4 * q + 1])), "f"(__uint_as_float(r[4 * q + 2])), "f"(__uint_as_float(r[4 * q + 3])) : "memory");
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (col + j < p.Cin) atomicAdd(out + c0 + j, __uint_as_float(r[j]));
-          }
-        }
-      }
-    }
+    wgmma_wait<0>();
+    if (any) wgrad_red<BN / 2>(acc, p.dW, p.Cout, p.Cin, tap, mt * 128, nt * BN);
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<(BN < 32 ? 32 : BN)>(tmem_base);
 }
 
 template <int BN>
@@ -195,9 +172,8 @@ static int launch_wgrad(const CUtensorMap& tmG, const CUtensorMap& tmX, const Wg
 // ------------------------------------------------------------------------------------------------ wgrad, NDHWC operands
 // The same GEMM read STRAIGHT from the NDHWC tensors (no channel-major copies): a TMA box (64 channels = 128 B, TW, TH, TT, TB)
 // of 64 positions lands in shared memory as 64 rows of 128 bytes — positions down the rows, 64 channels along each swizzled
-// row.  Read as an MN-MAJOR tcgen05 operand (instruction descriptor bits 15 / 16) that is exactly the canonical layout
-// ((8,8,m),(8,k)):((1,8,LBO),(64,SBO)) with K = the position axis: 8 positions x 128 B per swizzle atom (SBO = 1024 B between
-// 8-position groups) and LBO = 8 KB between 64-channel groups.  The filter tap is a coordinate shift of the input box (TMA
+// row.  Read as an MN-MAJOR wgmma operand (the transpose flags of the instruction) with K = the position axis: 8 positions
+// x 128 B per swizzle atom, 1024 B between 8-position groups.  The filter tap is a coordinate shift of the input box (TMA
 // zero fill = the conv's padding), exactly as in the forward kernel, so kw needs no pre-shifted copies.
 struct WgradNParams {
   int Cout, Cin, taps;
@@ -209,16 +185,6 @@ struct WgradNParams {
   float* dW;
 };
 
-__device__ __forceinline__ uint64_t make_sw128_mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;   // LBO: stride between 64-element groups along M / N
-  d |= (uint64_t)(1024 >> 4) << 32;                   // SBO: stride between 8-row groups along K
-  d |= (uint64_t)1 << 46;                             // version
-  d |= (uint64_t)2 << 61;                             // SWIZZLE_128B
-  return d;
-}
-
 template <int BN>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_nhwc_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmX, const WgradNParams p) {
@@ -227,21 +193,14 @@ wgrad_nhwc_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * ST_BYTES);
   uint64_t* empty = full + WG_STAGES;
-  uint64_t* acc_full = empty + WG_STAGES;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(acc_full + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();
     prefetch_tmap(&tmG); prefetch_tmap(&tmX);
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(acc_full, 1);
+    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], WG_CONSUMER_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<(BN < 32 ? 32 : BN)>(tmem_base_smem);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
 
   int w = blockIdx.x;
   const int ks = w % p.ksplit; w /= p.ksplit;
@@ -252,7 +211,7 @@ wgrad_nhwc_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant
   const int dw = kw - p.pW, dh = kh - p.pH, dt_ = kt - p.pT;
   const long long total = (long long)p.nN * p.nT * p.nH * p.nW;
   const long long k0 = total * ks / p.ksplit, k1 = total * (ks + 1) / p.ksplit;
-  // a k-block whose tap-shifted frames all lie outside the clip contributes zero: skipped by producer and issuer alike
+  // a k-block whose tap-shifted frames all lie outside the clip contributes zero: skipped by producer and consumers alike
   auto live = [&](int it) -> bool { const int t0 = it * p.TT + dt_; return t0 + p.TT > 0 && t0 < p.T; };
   auto decode = [&](long long kb, int& iw, int& ih, int& it, int& in) {
     iw = (int)(kb % p.nW); kb /= p.nW;
@@ -286,71 +245,49 @@ wgrad_nhwc_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant
       }
       if (++iw == p.nW) { iw = 0; if (++ih == p.nH) { ih = 0; if (++it == p.nT) { it = 0; ++in; } } }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc(128, BN, 1) | (1u << 15) | (1u << 16);      // A and B MN-major
+  } else if (warp >= 4) {
+    // Each 64-channel box is one MN-major swizzle atom wide; warpgroup g reads output-channel box g of the A stage and
+    // every input-channel box of the B stage, one m64n64k16 per (box, 16 positions = two 8-row groups 1024 B apart).
+    const uint32_t a_base = smem_u32(smem) + (uint32_t)((warp - 4) >> 2) * GRP;
     int stage = 0; uint32_t phase = 0;
     int iw, ih, it, in;
+    long long kb = k0;
     decode(k0, iw, ih, it, in);
+    auto skip_dead = [&]() {
+      while (kb < k1 && !live(it)) { ++kb; if (++iw == p.nW) { iw = 0; if (++ih == p.nH) { ih = 0; if (++it == p.nT) { it = 0; ++in; } } } }
+    };
+    skip_dead();
+    const bool any = kb < k1;
+    float acc[BN / 64][32];
+    int prev = -1;
     uint32_t first = 1;
-    for (long long kb = k0; kb < k1; ++kb) {
-      if (live(it)) {
-        mbar_wait(&full[stage], phase);
-        tcgen05_fence_after();
-        const uint32_t a_addr = smem_u32(smem) + stage * ST_BYTES;
-        if (elect_one()) {
+    while (kb < k1) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t a_addr = a_base + stage * ST_BYTES;
+      const uint32_t b_addr = smem_u32(smem) + stage * ST_BYTES + A_BYTES;
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {                                // 16 positions (2 swizzle atoms of 8 rows) per MMA
-            const uint64_t adesc = make_sw128_mnmajor_desc(a_addr + k * 2048, GRP);
-            const uint64_t bdesc = make_sw128_mnmajor_desc(a_addr + A_BYTES + k * 2048, GRP);
-            umma<false>(tmem_base, adesc, bdesc, idesc, (first && k == 0) ? 0u : 1u);
-          }
-          umma_commit(&empty[stage]);
-        }
-        first = 0;
-        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+      for (int k = 0; k < 4; ++k) {                                // 16 positions (2 swizzle atoms of 8 rows) per MMA
+        const uint64_t adesc = make_sw128_desc(a_addr + k * 2048, true);
+#pragma unroll
+        for (int g = 0; g < BN / 64; ++g)
+          wgmma<64, 0, 1>(acc[g], adesc, make_sw128_desc(b_addr + g * GRP + k * 2048, true), (first && k == 0) ? 0u : 1u);
       }
-      if (++iw == p.nW) { iw = 0; if (++ih == p.nH) { ih = 0; if (++it == p.nT) { it = 0; ++in; } } }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+      prev = stage;
+      first = 0;
+      if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+      ++kb; if (++iw == p.nW) { iw = 0; if (++ih == p.nH) { ih = 0; if (++it == p.nT) { it = 0; ++in; } } }
+      skip_dead();
     }
-    if (elect_one()) umma_commit(acc_full);
-  } else {
-    bool nothing = true;
-    {
-      int iw, ih, it, in;
-      decode(k0, iw, ih, it, in);
-      for (long long kb = k0; kb < k1 && nothing; ++kb) {
-        if (live(it)) nothing = false;
-        if (++iw == p.nW) { iw = 0; if (++ih == p.nH) { ih = 0; if (++it == p.nT) { it = 0; ++in; } } }
-      }
-    }
-    mbar_wait(acc_full, 0);
-    tcgen05_fence_after();
-    const int lg = warp & 3;
-    const int row = mt * 128 + lg * 32 + lane;
-    if (!nothing) {
-      float* out = p.dW + ((size_t)tap * p.Cout + row) * p.Cin + nt * BN;
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        uint32_t r[16];
-        tmem_ld_32x32b_x16(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)c0, r);
-        tmem_ld_wait();
-        if (row < p.Cout) {
-          const int col = nt * BN + c0;
-          if (col + 16 <= p.Cin && (p.Cin & 3) == 0) {
+    wgmma_wait<0>();
+    if (any) {
 #pragma unroll
-            for (int q = 0; q < 4; ++q)
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(out + c0 + 4 * q), "f"(__uint_as_float(r[4 * q])),
-                           "f"(__uint_as_float(r[4 * q + 1])), "f"(__uint_as_float(r[4 * q + 2])), "f"(__uint_as_float(r[4 * q + 3])) : "memory");
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (col + j < p.Cin) atomicAdd(out + c0 + j, __uint_as_float(r[j]));
-          }
-        }
-      }
+      for (int g = 0; g < BN / 64; ++g) wgrad_red<32>(acc[g], p.dW, p.Cout, p.Cin, tap, mt * 128, nt * BN + g * 64);
     }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<(BN < 32 ? 32 : BN)>(tmem_base);
 }
 
 template <int BN>
@@ -920,7 +857,7 @@ using namespace dt;
 
 static int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
-  const long long cap = 148ll * 16;
+  const long long cap = num_sms() * 16ll;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
@@ -957,11 +894,11 @@ extern "C" int dt_wgrad(const void* gz_planes, const void* x_planes, int N, int 
   memset(&p, 0, sizeof(p));
   p.Cout = Cout; p.Cin = Cin; p.taps = kT * kH * kW; p.kT = kT; p.kH = kH; p.kW = kW; p.pT = pT; p.pH = pH; p.pW = pW;
   p.Wp = Wp; p.T = T; p.N = N; p.kchunks = cdiv(plane, 64); p.dW = dW;
-  const int BN = Cin >= 256 ? 256 : (Cin > 64 ? 128 : 64);
+  const int BN = Cin > 64 ? 128 : 64;      // 128 x BN fp32 accumulators live in the registers of two warpgroups
   p.tiles_m = cdiv(Cout, 128); p.tiles_n = cdiv(Cin, BN);
   const long long units = (long long)p.taps * p.tiles_m * p.tiles_n;
   const long long kblocks = (long long)N * T * p.kchunks;
-  long long ksplit = (148 * 3 + units - 1) / units;               // ~3 waves of CTAs
+  long long ksplit = (num_sms() * 3ll + units - 1) / units;               // ~3 waves of CTAs
   if (ksplit > kblocks / 4) ksplit = kblocks / 4;
   if (ksplit < 1) ksplit = 1;
   p.ksplit = (int)ksplit;
@@ -979,7 +916,6 @@ extern "C" int dt_wgrad(const void* gz_planes, const void* x_planes, int N, int 
     if (encode_map(&tmX, 0, 5, x_planes, d, s, b, e)) return 1;
   }
   switch (BN) {
-    case 256: return launch_wgrad<256>(tmG, tmX, p, stream);
     case 128: return launch_wgrad<128>(tmG, tmX, p, stream);
     default: return launch_wgrad<64>(tmG, tmX, p, stream);
   }
@@ -1013,17 +949,17 @@ extern "C" int dt_wgrad_nhwc(const void* gz, int ld_g, const void* x, int ld_x, 
         }
   }
   p.nW = cdiv(Wo, p.TW); p.nH = cdiv(Ho, p.TH); p.nT = cdiv(T, p.TT); p.nN = cdiv(N, p.TB);
-  const int BN = Cin >= 256 ? 256 : (Cin > 64 ? 128 : 64);
+  const int BN = Cin > 64 ? 128 : 64;      // 128 x BN fp32 accumulators live in the registers of two warpgroups
   p.tiles_m = cdiv(Cout, 128); p.tiles_n = cdiv(Cin, BN);
   const long long units = (long long)p.taps * p.tiles_m * p.tiles_n;
   const long long kblocks = (long long)p.nW * p.nH * p.nT * p.nN;
   // K split: every CTA adds its 128 x BN partial tile into dW with red.global, so the split count is also the atomic
   // traffic multiplier.  DT_WGRAD_WAVES overrides the wave count (tuning knob of tools/bench_wgrad.py).
-  // Measured on B200 (tools/bench_wgrad.py, profiles/wgrad_waves_r02.md): pointwise layers are fastest with ONE wave of CTAs
-  // (a 1x1 filter has few (tap, tile) units, so 3 waves meant ~100 partial tiles added per output tile), multi-tap layers with 2.
+  // Pointwise layers use ONE wave of CTAs (a 1x1 filter has few (tap, tile) units, so more waves mean many partial tiles
+  // added per output tile), multi-tap layers two.
   static const int waves_env = [] { const char* e = getenv("DT_WGRAD_WAVES"); const int v = e ? atoi(e) : 0; return v >= 1 && v <= 16 ? v : 0; }();
   const int waves = waves_env ? waves_env : (p.taps == 1 ? 1 : 2);
-  long long ksplit = (148 * waves + units - 1) / units;
+  long long ksplit = ((long long)num_sms() * waves + units - 1) / units;
   if (ksplit > kblocks / 4) ksplit = kblocks / 4;
   if (ksplit < 1) ksplit = 1;
   p.ksplit = (int)ksplit;
@@ -1042,7 +978,6 @@ extern "C" int dt_wgrad_nhwc(const void* gz, int ld_g, const void* x, int ld_x, 
     if (encode_map(&tmX, 0, 5, x, d, st, box, e)) return 1;
   }
   switch (BN) {
-    case 256: return launch_wgrad_nhwc<256>(tmG, tmX, p, stream);
     case 128: return launch_wgrad_nhwc<128>(tmG, tmX, p, stream);
     default: return launch_wgrad_nhwc<64>(tmG, tmX, p, stream);
   }
@@ -1120,7 +1055,7 @@ extern "C" int dt_bias_grad(const void* g, long long rows, int C, int ld, float*
   DT_CHECK_ARG(rows >= 0 && C >= 8 && C % 8 == 0 && ld >= C && ld % 8 == 0, "dt_bias_grad: bad shape rows=%lld C=%d ld=%d (multiples of 8)", rows, C, ld);
   if (rows == 0) return 0;
   DT_CHECK_ARG(g && db, "dt_bias_grad: null pointer");
-  long long gx = rows / 128; if (gx < 1) gx = 1; if (gx > 148 * 8) gx = 148 * 8;
+  long long gx = rows / 128; if (gx < 1) gx = 1; if (gx > num_sms() * 8ll) gx = num_sms() * 8ll;
   dim3 grid((unsigned)gx, (C + 255) / 256);
   bias_grad_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)g, rows, C, ld, db);
   DT_CHECK_LAUNCH();

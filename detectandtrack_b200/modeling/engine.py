@@ -1,10 +1,10 @@
-"""B200 execution engine for the reference's keypoint R-CNN graphs.
+"""H100 execution engine for the reference's keypoint R-CNN graphs.
 
 What the reference runs as three Caffe2 nets with host ops in between
 (lib/core/test.py:158-252,584-627,897-958; SURVEY.md §3.1) runs here as one stream of
 kernel launches with no host round trip between the image blob and the detections:
 
-  prep_clip -> conv1 -> pool1 -> res2..res5 (tcgen05 implicit GEMM, fused affine/ReLU/residual)
+  prep_clip -> conv1 -> pool1 -> res2..res5 (wgmma implicit GEMM, fused affine/ReLU/residual)
   -> FPN (lateral 1x1 with the top-down upsample-add in the epilogue, post-hoc convs, P6)
   -> [body/head link: centre-frame slice]
   -> per level: RPN 3x3 + fused (cls|bbox) 1x1 -> device top-k/decode -> batched bitmask NMS

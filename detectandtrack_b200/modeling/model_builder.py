@@ -2,7 +2,7 @@
 
 The reference resolves MODEL.TYPE to a graph-building function and returns a
 DetectionModelHelper holding Caffe2 nets (``net``, ``conv_body_net``, ``keypoint_net``).
-Here the returned object is a ``DetectionModel`` wrapping the B200 ``DetectionEngine``; the
+Here the returned object is a ``DetectionModel`` wrapping the H100 ``DetectionEngine``; the
 three "nets" are methods on it with the same split the reference makes for inference
 (:179-306): bbox net (body + RPN + box head), conv-body net, keypoint net.
 """

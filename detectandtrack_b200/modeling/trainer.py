@@ -6,7 +6,7 @@ Implemented graph: the reference's RPN training model (``MODEL.TYPE rpn``, model
 frozen (freeze_at=2, ResNet3D.py:273-274; AffineChannel parameters frozen everywhere), res3..res5 + FPN + RPN heads
 trained: forward in bf16 (fp32 accumulate), backward =
     dgrad   dt_conv3d with the flipped / transposed filter (+ dt_scatter_stride2 for the stride-2 1x1 convs)
-    wgrad   dt_wgrad on channel-major planes (tcgen05, split-K)
+    wgrad   dt_wgrad on channel-major planes (wgmma, split-K)
     joins   dt_bwd_pointwise (Relu / Sum / AffineChannelNd gradients), dt_upsample_add_bwd (FPN top-down), dt_bias_grad
     losses  dt_rpn_loss_grad per level (SigmoidCrossEntropyLoss + SmoothL1Loss)
 then a bucketed gradient SUM all-reduce over NCCL issued per bucket as soon as its filter gradients are enqueued
@@ -131,7 +131,7 @@ class TrainConv(object):
             if x_planes is None:
                 x_planes = to.to_planes(x, pad=sp, stride=self.stride[1:], channels=self.cin, copies=True)
             to.wgrad(to.to_planes(gz, pad=sp), x_planes, (Ho, Wo), self.k, self.g)
-        else:                 # operands read straight from NDHWC (MN-major tcgen05 operands, tap = TMA coordinate shift)
+        else:                 # operands read straight from NDHWC (MN-major wgmma operands, tap = TMA coordinate shift)
             to.wgrad_nhwc(gz, x, self.k, self.stride[1:], self.g, cout=self.cout, cin=self.cin)
         if self.bias is not None:
             L.call('dt_bias_grad', L.ptr(gz), gz.numel() // gz.shape[-1], self.cout, gz.shape[-1], L.ptr(self.bias_g), L.stream_ptr())

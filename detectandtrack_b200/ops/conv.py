@@ -1,4 +1,4 @@
-"""Device-tensor API over csrc/conv_tc.cu (tcgen05 implicit-GEMM Conv3d/Conv2d/FC).
+"""Device-tensor API over csrc/conv_tc.cu (wgmma implicit-GEMM Conv3d/Conv2d/FC).
 Tensors are NDHWC ([N, T, H, W, C], channels innermost); torch is only the memory
 container.  See include/dt_b200.h (dt_conv_desc / dt_conv3d) for the contract."""
 import ctypes as C
@@ -81,8 +81,8 @@ def join_tf32(t):
 
 
 def round_tf32(t):
-    """Round an fp32 tensor to the nearest (even) tf32-representable value.  tcgen05 kind::tf32
-    truncates the low 13 mantissa bits of its operands; feeding it pre-rounded values makes the
+    """Round an fp32 tensor to the nearest (even) tf32-representable value.  The tf32 MMA
+    ignores the low 13 mantissa bits of its operands; feeding it pre-rounded values makes the
     truncation exact instead of a one-sided error."""
     torch = L.require_cuda()
     u = t.contiguous().view(torch.int32)

@@ -1,4 +1,4 @@
-/* dt_b200.h — C ABI of libdt_b200.so, the B200 (sm_100a) hot path behind the
+/* dt_b200.h — C ABI of libdt_b200.so, the H100 (sm_90a) hot path behind the
  * DetectAndTrack cfg / model-builder / tools surface.
  *
  * Conventions (all entry points):
@@ -128,8 +128,8 @@ int dt_prune_detections(const float* boxes, int nframes, int dmax, int ld, int T
 
 /* ---- conv_tc.cu ---------------------------------------------------------- */
 
-#define DT_DTYPE_BF16 0   /* bf16 activations/weights, fp32 accumulate (tcgen05 kind::f16)   */
-#define DT_DTYPE_TF32 1   /* fp32 storage, tf32 multiply, fp32 accumulate (tcgen05 kind::tf32) */
+#define DT_DTYPE_BF16 0   /* bf16 activations/weights, fp32 accumulate (wgmma .bf16)         */
+#define DT_DTYPE_TF32 1   /* fp32 storage, tf32 multiply, fp32 accumulate (wgmma .tf32)         */
 #define DT_DTYPE_F16 2    /* fp16 x and w (11-bit operands at the full kind::f16 rate), fp32 accumulate; plain rows, no residual;
                              y is bf16 / bf16 pairs (x3 bit 1) / fp32 as for DT_DTYPE_BF16 */
 
@@ -353,7 +353,7 @@ int dt_wgrad(const void* gz_planes, const void* x_planes, int N, int T, int Ho, 
              float* dW, void* stream);
 
 /* The same filter gradient read straight from the NDHWC tensors (no planes): gz [N, T, Ho, Wo, ld_g] (first Cout channels),
- * x [N, T, Hi, Wi, ld_x] (first Cin channels), both bf16.  Positions are the K axis of MN-major tcgen05 operands staged by
+ * x [N, T, Hi, Wi, ld_x] (first Cin channels), both bf16.  Positions are the K axis of MN-major wgmma operands staged by
  * 5-D TMA boxes; the tap is a coordinate shift (zero fill = padding).  sH / sW > 1 only for pointwise convs
  * (Ho = ceil(Hi / sH)).  dW [taps][Cout][Cin] fp32 is accumulated into (caller zeroes). */
 int dt_wgrad_nhwc(const void* gz, int ld_g, const void* x, int ld_x, int N, int T, int Ho, int Wo, int Hi, int Wi, int Cout, int Cin,

@@ -233,6 +233,22 @@ def main():
         r, c = scipy.optimize.linear_sum_assignment(C)
         out['lsa_C_' + nm], out['lsa_r_' + nm], out['lsa_c_' + nm] = C, r, c
 
+    # the compiled reference Cython itself on the seeded inputs of tests/test_oracle_boxes.py (*_vs_compiled_reference)
+    from oracle._ref import cython_bbox, cython_nms
+    rng = np.random.default_rng(5)
+    for i, scale in enumerate((0.02, 1.0, 7.0)):
+        x1 = rng.uniform(0, 500, 400); y1 = rng.uniform(0, 300, 400)
+        a = np.stack([x1, y1, x1 + rng.uniform(0, 200, 400) * scale, y1 + rng.uniform(0, 200, 400) * scale], 1).astype(np.float32)
+        out['refcy_iou_boxes_%d' % i], out['refcy_iou_out_%d' % i] = a, cython_bbox.bbox_overlaps(a[:250], a[250:])
+    rng = np.random.default_rng(7)
+    c = rng.uniform(0, 600, (60, 2))
+    xy = c[rng.integers(0, 60, 1500)] + rng.normal(0, 12, (1500, 2))
+    wh = rng.uniform(20, 120, (1500, 2))
+    d = np.hstack([xy, xy + wh, rng.permutation(1500)[:, None] / 1500.]).astype(np.float32)
+    out['refcy_nms_dets'] = d
+    for th in (0.3, 0.7):
+        out['refcy_nms_keep_%d' % int(th * 10)] = np.asarray(cython_nms.nms(d, np.float32(th)), dtype=np.int64)
+
     groups = {}
     for k, v in out.items():
         groups.setdefault(k.split('_')[0], {})[k] = np.asarray(v)

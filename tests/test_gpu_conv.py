@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM convolution (through the C ABI) against a plain
+"""GPU parity of the wgmma implicit-GEMM convolution (through the C ABI) against a plain
 PyTorch fp32 reference of the same op (torch.nn.functional.conv3d on the CPU, the stand-in
 for the un-vendored Caffe2 ConvNd + AffineChannelNd + Sum + Relu; "parity unpinned" by the
 reference, SURVEY.md §8c).

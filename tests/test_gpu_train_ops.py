@@ -187,7 +187,7 @@ NHWC_CASES = WG_CASES + [
 
 @pytest.mark.parametrize('case', range(len(NHWC_CASES)))
 def test_wgrad_nhwc_vs_autograd(case):
-    """dt_wgrad_nhwc (operands straight from NDHWC as MN-major tcgen05 operands) against torch autograd in fp32."""
+    """dt_wgrad_nhwc (operands straight from NDHWC as MN-major wgmma operands) against torch autograd in fp32."""
     import torch
     import torch.nn.functional as F
     N, T, H, W, Cin, Cout, k = NHWC_CASES[case]

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 conv kernel on the layer shapes that dominate the
+"""Micro-benchmark of the wgmma conv kernel on the layer shapes that dominate the
 R50-FPN-3D clip (SURVEY.md §8d).  CUDA-event timing, L2 flushed between iterations.
     python tools/bench_conv.py [--dtype bf16|tf32|bf16x3|tf32x3] [--iters 5]
 (split modes: [hi | lo] pair inputs / outputs, 3 MMAs per k-block; TFLOP/s are ALGORITHMIC: 2*MACs of the fp32 conv)

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 filter-gradient kernels on the trainable layer shapes of the keypoint R-CNN training step at
+"""Micro-benchmark of the wgmma filter-gradient kernels on the trainable layer shapes of the keypoint R-CNN training step at
 TRAIN.IMS_PER_BATCH = 2 clips (T = 3, 800x1344 blob): dt_wgrad_nhwc (operands straight from NDHWC, the path the trainer uses)
 next to the first implementation (dt_to_planes + dt_wgrad).  CUDA events, median of --iters; TFLOP/s = 2*MACs of the conv.
     python tools/bench_wgrad.py [--iters 5] [--only res4] [--planes]"""
