@@ -104,7 +104,7 @@ class ConvDesc(C.Structure):
 class ConvPlan(C.Structure):
     """dt_conv_plan_t (include/dt_b200.h)."""
     _fields_ = [(n, C.c_int) for n in ('BN', 'TH', 'TW', 'TT', 'TB', 'tiles', 'kiters', 'stages', 'ks', 'ncbuf', 'nrbuf',
-                                        'smem_bytes')] + [('useful_rows', C.c_double)]
+                                        'smem_bytes')] + [('useful_rows', C.c_double), ('stage_bytes', C.c_int)]
 
 
 _RESTYPE = {'dt_last_error': C.c_char_p}

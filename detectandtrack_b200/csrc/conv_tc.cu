@@ -73,15 +73,14 @@ struct ConvKernelParams {
   int out_f32;                 // 1: fp32 output, 0: bf16
   // 3xTF32 ("fp32-accurate") mode: activations / weights are stored as [hi | lo] tf32 pairs along the
   // channel axis; D = A_hi*B_hi + A_lo*B_hi + A_hi*B_lo (the lo*lo term is below fp32 resolution).
-  int split_in;                // 1: three k-blocks per (tap, channel chunk) with the offsets below
-  int nsub;                    // k-blocks per (tap, channel chunk): 1 plain, 3 split operands (hi*hi, lo*hi, hi*lo),
-                               // 2 split conv1 (the blob pixel carries [hi3 | lo3]: one block against [W_hi | W_hi], one against [W_lo | 0])
+  int split_in;                // 1: x and w rows are [hi | lo] pairs with the offsets below (kernel NMMA = 3)
   int a_lo_off, b_lo_off;      // element offsets of the lo halves in the x rows / packed weight rows
+  int b_lo_blk;                // split conv1: the lo weight box is the next packed weight block instead
   int split_out;               // 1: write hi at channel c and lo at out_lo_off + c (fp32)
   int out_lo_off, res_lo_off;  // lo-half offsets of the output / residual rows
   int nstages, ncbuf;          // smem split chosen per layer: operand ring depth / output staging buffers
-  int ks;                      // k-blocks per ring stage
-  int ktab;                    // entries of the k-block schedule (kiters + 1 padding, even)
+  int ks;                      // (tap, channel chunk) groups per ring stage
+  int ktab;                    // entries of the schedule (one per group + 1 padding, even)
   int t_first;                 // first output frame computed (frames before it are skipped)
   int row_planes;              // conv1: input rows de-interleaved by parity, filter row kh -> plane kh & 1, row + kh >> 1
   int nrbuf;                   // > 0: bf16 residual chunks arrive by TMA in a ring of this many staged chunks
@@ -107,31 +106,50 @@ template <int BN>
 struct ConvCfg {
   static constexpr int A_BYTES = 128 * 128;            // 128 rows x 128 B
   static constexpr int B_BYTES = BN * 128;
-  static constexpr int KB_BYTES = A_BYTES + B_BYTES;   // one k-block of both operands
   static constexpr int MAX_STAGES = 8;
   static constexpr int C_BYTES = 128 * 128;            // one staged output chunk: 128 rows x 128 B
   static constexpr int BAR_BYTES = 384;                // mbarriers
   static constexpr int FIXED_BYTES = BAR_BYTES;
   static constexpr int BUDGET = 227 * 1024;
+  // A (tap, channel chunk) group of a conv with nmma MMA k-blocks per group is its activation boxes followed by its
+  // weight boxes, each fetched once: plain [A | W]; split operands (nmma 3) [A_hi A_lo | W_hi W_lo] for the products
+  // A_hi*W_hi, A_lo*W_hi, A_hi*W_lo; split conv1 (nmma 2) [A | W_2kh W_2kh+1] (the blob pixel carries [hi3 | lo3]:
+  // block 2*kh is [W_hi | W_hi], block 2*kh + 1 is [W_lo | 0]).
+  static constexpr int boxes_a(int nmma) { return nmma == 3 ? 2 : 1; }
+  static constexpr int boxes_b(int nmma) { return nmma >= 2 ? 2 : 1; }
+  static constexpr int group_bytes(int nmma) { return boxes_a(nmma) * A_BYTES + boxes_b(nmma) * B_BYTES; }
   // K-heavy layers want a deep operand ring; K-light (HBM-bound) layers want output staging buffers so the
   // epilogue never waits for a TMA store to drain, and (with a residual) a ring of prefetched residual chunks.
-  static int tab_bytes(int kiters) { return ((kiters + 2) * 24 + 127) / 128 * 128; }   // k-block schedule
-  static void split(int kiters, bool res_tma, bool split_out, bool out_f32, int* stages, int* ks, int* ncbuf, int* nrbuf) {
+  static int tab_bytes(int groups) { return ((groups + 2) * 24 + 127) / 128 * 128; }   // schedule: one entry per group
+  static void split(int groups, int nmma, bool res_tma, bool split_out, bool out_f32, int* stages, int* ks, int* ncbuf,
+                    int* nrbuf) {
+    const int kiters = groups * nmma;                   // MMA k-blocks per tile
+    const int gb = group_bytes(nmma);
     const int chunks = BN / (out_f32 ? 32 : 64);        // staged chunks per tile
     int c = (kiters >= 12 && !split_out) ? 2 : 4;       // split (hi, lo) output: two slots of two buffers
     if (!split_out && c > 2 * chunks) c = chunks >= 1 ? 2 * chunks : 2;   // two tiles of staging are enough
-    const int r = res_tma ? ((kiters >= 12 || split_out) ? 2 : 4) : 0;      // split output: a residual slot is a chunk pair
+    int r = res_tma ? ((kiters >= 12 || split_out) ? 2 : 4) : 0;      // split output: a residual slot is a chunk pair
+    const int fixed = BUDGET - FIXED_BYTES - tab_bytes(groups);
+    // split stages (64 KiB at BN = 128) need room.  The split residual layers fit two stages by keeping one residual
+    // slot pair instead of two (measured faster than giving up an output staging slot pair instead)
+    if (split_out && nmma > 1 && r > 1 && (fixed - (c + 2 * r) * C_BYTES) / gb < 2) r = 1;
     const int rb = split_out ? 2 * r : r;
+    // with two split stages only one group's refill is in flight while the other's MMAs run, and a 64 KiB refill does
+    // not land within one group's MMA time: a K-heavy split output is staged through one (hi, lo) slot pair instead of
+    // two when that buys a third stage (K-light layers measured faster with both slot pairs)
+    const int st_wide = (fixed - (c + rb) * C_BYTES) / gb, st_lean = (fixed - (2 + rb) * C_BYTES) / gb;
+    if (split_out && nmma > 1 && c > 2 && kiters >= 12 && st_wide < 3 && st_lean > st_wide) c = 2;
     // narrow tiles retire a k-block's MMAs faster than one producer / issuer round trip through the
-    // mbarriers: let a ring stage carry two k-blocks there (same bytes in flight, half the handshakes)
-    const int avail = BUDGET - FIXED_BYTES - tab_bytes(kiters) - (c + rb) * C_BYTES;
-    const int k = (BN <= 128 && kiters >= 2 && avail / (2 * KB_BYTES) >= 3) ? 2 : 1;
-    int st = avail / (k * KB_BYTES);
+    // mbarriers: let a ring stage carry two plain k-blocks there (same bytes in flight, half the handshakes)
+    const int avail = fixed - (c + rb) * C_BYTES;
+    const int k = (nmma == 1 && BN <= 128 && kiters >= 2 && avail / (2 * gb) >= 3) ? 2 : 1;
+    int st = avail / (k * gb);
     if (st > MAX_STAGES) st = MAX_STAGES;
     *stages = st; *ks = k; *ncbuf = c; *nrbuf = r;
   }
-  static int smem_bytes(int kiters, int stages, int ks, int ncbuf, int nrbuf, bool split_out) {
-    return stages * ks * KB_BYTES + (ncbuf + (split_out ? 2 : 1) * nrbuf) * C_BYTES + FIXED_BYTES + tab_bytes(kiters);
+  static int smem_bytes(int groups, int nmma, int stages, int ks, int ncbuf, int nrbuf, bool split_out) {
+    return stages * ks * group_bytes(nmma) + (ncbuf + (split_out ? 2 : 1) * nrbuf) * C_BYTES + FIXED_BYTES +
+           tab_bytes(groups);
   }
 };
 
@@ -149,7 +167,9 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvKernelParams& p, int 
 // SPLIT: the output (and the residual) rows are [hi | lo] pairs (the x3 modes' intermediate activations); a template
 // parameter so that the plain kernels do not carry the pair logic's registers.
 // KIND: MMA operand type, 0 bf16, 1 fp16, 2 tf32 (wgmma.cuh).
-template <int BN, int KIND, bool SPLIT>
+// NMMA: MMA k-blocks per (tap, channel chunk) group, 1 plain, 3 split operands, 2 split conv1 (ConvCfg::group_bytes);
+// a template parameter so that the products of a group are straight-line wgmmas.
+template <int BN, int KIND, bool SPLIT, int NMMA>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
@@ -157,10 +177,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   using Cfg = ConvCfg<BN>;
   const int STAGES = p.nstages;
   constexpr int BK = KIND == 2 ? 32 : 64;            // elements per 128-byte k-block
+  constexpr int NA = Cfg::boxes_a(NMMA), NB = Cfg::boxes_b(NMMA);
   // SWIZZLE_128B operands need 1024-byte aligned tiles: the dynamic window is declared with that alignment
   // (no static shared memory in this kernel) and checked once below instead of spending a kilobyte on slack
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* cbuf = smem + STAGES * p.ks * Cfg::KB_BYTES;              // [NCBUF][128 rows][128 B], 128B-swizzled
+  // ring stage: p.ks groups of [A_0 .. A_{NA-1} | W_0 .. W_{NB-1}], every box 1024-byte aligned
+  constexpr uint32_t group_bytes = (uint32_t)Cfg::group_bytes(NMMA);
+  const uint32_t stage_bytes = (uint32_t)p.ks * group_bytes;
+  uint8_t* cbuf = smem + STAGES * stage_bytes;                       // [NCBUF][128 rows][128 B], 128B-swizzled
   uint8_t* rbuf = cbuf + p.ncbuf * Cfg::C_BYTES;                     // [NRBUF] residual chunks, same layout
   constexpr uint32_t rslot_bytes = SPLIT ? 2u * Cfg::C_BYTES : (uint32_t)Cfg::C_BYTES;   // split: (hi, lo) chunk pair
   uint64_t* bars = reinterpret_cast<uint64_t*>(rbuf + p.nrbuf * rslot_bytes);
@@ -170,33 +194,28 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* r_empty = r_full + 4;              // [4]       residual chunk consumed
   uint64_t* c_full = r_full + 8;               // [4]       output chunk staged by all epilogue warps
   uint64_t* c_free = r_full + 12;              // [4]       staging slot read out by its TMA store
-  // k-block schedule of one tile: what the producers add to the tile's base coordinates for k-block j.
+  // schedule of one tile, one entry per (tap, channel chunk) group: what the producers add to the tile's base
+  // coordinates for the group's first boxes (its lo boxes sit at the lo offsets from there).
   // Built once; walking taps / channel chunks with carry logic in the producer loop costs more cycles per
   // k-block than a narrow tile's MMAs take.
   int4* tabA = reinterpret_cast<int4*>(reinterpret_cast<uint8_t*>(bars) + Cfg::BAR_BYTES);   // {c, dw, dh, dt}
-  int2* tabB = reinterpret_cast<int2*>(tabA + p.ktab);                                        // {c, tap}
+  int2* tabB = reinterpret_cast<int2*>(tabA + p.ktab);                                        // {c, weight block}
   if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();
   {
-    const int nsub = p.nsub;
-    const int kit = p.kT * p.kH * p.kW * p.kchunks * nsub;
+    const int groups = p.kT * p.kH * p.kW * p.kchunks;
     for (int j = threadIdx.x; j < p.ktab; j += blockDim.x) {
-      const int jj = min(j, kit - 1);                   // padding entries repeat the last k-block (never issued)
-      const int sub = jj % nsub;
-      int r = jj / nsub;
+      int r = min(j, groups - 1);                       // padding entries repeat the last group (never issued)
       const int kc = r % p.kchunks; r /= p.kchunks;
       const int tap = r;
       const int kw = r % p.kW; r /= p.kW;
       const int kh = r % p.kH;
       const int kt = r / p.kH;
-      // sub 0: A_hi x B_hi, 1: A_lo x B_hi, 2: A_hi x B_lo
-      const int ca = kc * BK + (sub == 1 ? p.a_lo_off : 0);
-      const int cb = kc * BK + (sub == 2 ? p.b_lo_off : 0);
       if (p.row_planes) {          // conv1: one box per filter row; split mode: weight blocks 2*kh (hi) and 2*kh + 1 (lo)
         tabA[j] = make_int4(0, 0, kh >> 1, kh & 1);
-        tabB[j] = make_int2(0, tap * nsub + sub);
+        tabB[j] = make_int2(0, tap * NB);
       } else {
-        tabA[j] = make_int4(ca, kw, kh, kt);
-        tabB[j] = make_int2(cb, tap);
+        tabA[j] = make_int4(kc * BK, kw, kh, kt);
+        tabB[j] = make_int2(kc * BK, tap);
       }
     }
   }
@@ -224,8 +243,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  const int taps = p.kT * p.kH * p.kW;
-  const int kiters = taps * p.kchunks * p.nsub;
+  const int groups = p.kT * p.kH * p.kW * p.kchunks;    // (tap, channel chunk) groups per tile
 
   if (warp == 0 || warp == B_WARP) {
     // ===================== TMA producers =====================
@@ -236,11 +254,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const bool load_b = warp != 0;
     int stage = 0; uint32_t phase = 0;
     int rslot = 0; uint32_t rphase = 0;
-    const uint32_t smem_u = smem_u32(smem) + (load_b ? (uint32_t)Cfg::A_BYTES : 0u);
+    const uint32_t smem_u = smem_u32(smem) + (load_b ? (uint32_t)(NA * Cfg::A_BYTES) : 0u);
     const uint32_t full_u = smem_u32(full), empty_u = smem_u32(empty);
-    const int KS = p.ks;                                  // k-blocks per ring stage (one mbarrier round trip)
-    const uint32_t stage_bytes = (uint32_t)KS * Cfg::KB_BYTES;
-    const uint32_t kb_tx = load_b ? (uint32_t)Cfg::B_BYTES : p.a_bytes;
+    const int KS = p.ks;                                  // groups per ring stage (one mbarrier round trip)
+    const int nbox = load_b ? NB : NA;                    // this warp's boxes per group: hi, then lo
+    const uint32_t box_bytes = load_b ? (uint32_t)Cfg::B_BYTES : (uint32_t)Cfg::A_BYTES;
+    const uint32_t box_tx = load_b ? (uint32_t)Cfg::B_BYTES : p.a_bytes;
+    const int lo_c = load_b ? p.b_lo_off : p.a_lo_off;    // the lo box: channel offset / weight block offset
+    const int lo_blk = load_b ? p.b_lo_blk : 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const TileCoord tc = decode_tile(p, tile);
       const int n = tc.tbi * p.TB;
@@ -248,9 +269,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int h_base = tc.thi * p.TH * p.sH - p.pH;
       const int t_base = p.row_planes ? 0 : (tc.tti * p.TT + p.t_first) * p.sT - p.pT;
       const int n_base = tc.nt * BN;
-      for (int ki = 0; ki < kiters; ki += KS) {
-        const int nk = min(KS, kiters - ki);
-        // this stage's k-blocks from the schedule (uniform loads), then ONE elected issue block
+      for (int ki = 0; ki < groups; ki += KS) {
+        const int nk = min(KS, groups - ki);
+        // this stage's groups from the schedule (uniform loads), then ONE elected issue block
         int x0[2], x1[2], x2[2], x3[2];
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
@@ -266,13 +287,16 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (elect_one()) {
           const uint32_t bar = full_u + stage * 8;
           const uint32_t dst = smem_u + stage * stage_bytes;
-          mbar_expect_tx_u(bar, (uint32_t)nk * kb_tx);
-          if (load_b) {
-            tma_load_3d_u(dst, &tmB, bar, x0[0], x1[0], x2[0]);
-            if (nk > 1) tma_load_3d_u(dst + Cfg::KB_BYTES, &tmB, bar, x0[1], x1[1], x2[1]);
-          } else {
-            tma_load_5d_u(dst, &tmA, bar, x0[0], x1[0], x2[0], x3[0], n);
-            if (nk > 1) tma_load_5d_u(dst + Cfg::KB_BYTES, &tmA, bar, x0[1], x1[1], x2[1], x3[1], n);
+          mbar_expect_tx_u(bar, (uint32_t)(nk * nbox) * box_tx);
+#pragma unroll
+          for (int q = 0; q < 2; ++q) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              if (q >= nk || i >= nbox) continue;
+              const uint32_t d = dst + q * group_bytes + i * box_bytes;
+              if (load_b) tma_load_3d_u(d, &tmB, bar, x0[q] + i * lo_c, x1[q], x2[q] + i * lo_blk);
+              else tma_load_5d_u(d, &tmA, bar, x0[q] + i * lo_c, x1[q], x2[q], x3[q], n);
+            }
           }
         }
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -379,29 +403,34 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const uint32_t smem_u = smem_u32(smem) + (uint32_t)wg * (64u * 128u);   // this warpgroup's 64 rows of the A tile
     const uint32_t full_u = smem_u32(full);
     const int KS = p.ks;
-    const uint32_t stage_bytes = (uint32_t)KS * Cfg::KB_BYTES;
     int stage = 0; uint32_t phase = 0;
     int rslot = 0; uint32_t rphase = 0;
     int slot = 0; uint32_t sphase = 0;
     float acc[BN / 2];
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const TileCoord tc = decode_tile(p, tile);
-      // ---- main loop: one wgmma group per k-block; a ring stage goes back to the producers once the group of the
-      // NEXT stage's last k-block is issued and the stage's own groups retired (one stage stays in flight).  The
-      // wgmmas sit outside any branch so that they are not serialized.
+      // ---- main loop: one wgmma group per (tap, channel chunk) group; a ring stage goes back to the producers once
+      // the wgmma group of the NEXT stage's last group is issued and the stage's own wgmma groups retired (one stage
+      // stays in flight).  The wgmmas sit outside any branch so that they are not serialized.
       int prev = -1;
-      for (int ki = 0; ki < kiters; ++ki) {
-        const int q = KS == 2 ? (ki & 1) : 0;          // k-block inside the ring stage
+      for (int ki = 0; ki < groups; ++ki) {
+        const int q = KS == 2 ? (ki & 1) : 0;          // group inside the ring stage
         if (q == 0) mbar_wait_u(full_u + stage * 8, phase);
-        const uint32_t off = stage * stage_bytes + q * Cfg::KB_BYTES;
-        const uint64_t adesc = make_sw128_desc(smem_u + off);
-        const uint64_t bdesc = make_sw128_desc(smem_u32(smem) + off + Cfg::A_BYTES);
+        const uint32_t off = stage * stage_bytes + q * group_bytes;
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k)                    // 4 x 32 B = one 128-byte swizzle row of K
-          wgmma<BN, KIND>(acc, adesc + 2 * k, bdesc + 2 * k, (ki | k) != 0 ? 1u : 0u);
+        for (int s = 0; s < NMMA; ++s) {
+          // products in a fixed order: A_0 W_0, then A_1 W_0 (split), then A_0 W_1 (split, split conv1)
+          const uint32_t ai = (NA == 2 && s == 1) ? 1u : 0u;
+          const uint32_t bi = (NB == 2 && s == NMMA - 1) ? 1u : 0u;
+          const uint64_t adesc = make_sw128_desc(smem_u + off + ai * Cfg::A_BYTES);
+          const uint64_t bdesc = make_sw128_desc(smem_u32(smem) + off + NA * Cfg::A_BYTES + bi * Cfg::B_BYTES);
+#pragma unroll
+          for (int k = 0; k < 4; ++k)                  // 4 x 32 B = one 128-byte swizzle row of K
+            wgmma<BN, KIND>(acc, adesc + 2 * k, bdesc + 2 * k, (ki | s | k) != 0 ? 1u : 0u);
+        }
         wgmma_commit();
-        if (q == KS - 1 || ki == kiters - 1) {
+        if (q == KS - 1 || ki == groups - 1) {
           if (q == 1) wgmma_wait<2>(); else wgmma_wait<1>();   // only this stage's q + 1 groups may still run
           if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
           prev = stage;
@@ -571,18 +600,18 @@ static int encode_out_map(CUtensorMap* m, void* y, int out_f32, int Cout, int Wo
   return encode_map(m, out_f32 != 0 ? 1 : 0, 5, y, d, st, b, e);
 }
 
-template <int BN, int KIND, bool SPLIT>
+template <int BN, int KIND, bool SPLIT, int NMMA>
 static int launch_conv1(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
                        const ConvKernelParams& p, int grid, cudaStream_t stream) {
   using Cfg = ConvCfg<BN>;
   static DynSmemGrant grant;
-  DT_CHECK_CUDA(grant_dyn_smem(conv_tc_kernel<BN, KIND, SPLIT>, Cfg::BUDGET, &grant));
+  DT_CHECK_CUDA(grant_dyn_smem(conv_tc_kernel<BN, KIND, SPLIT, NMMA>, Cfg::BUDGET, &grant));
   ConvKernelParams q = p;
-  const int kiters = p.kT * p.kH * p.kW * p.kchunks * p.nsub;
-  DT_CHECK_ARG(kiters <= 2048, "conv: %d k-blocks per tile exceed the schedule table", kiters);
-  Cfg::split(kiters, p.nrbuf > 0, p.split_out != 0, p.out_f32 != 0, &q.nstages, &q.ks, &q.ncbuf, &q.nrbuf);
-  q.ktab = (kiters + 2) & ~1;
-  const int smem = Cfg::smem_bytes(kiters, q.nstages, q.ks, q.ncbuf, q.nrbuf, p.split_out != 0);
+  const int groups = p.kT * p.kH * p.kW * p.kchunks;
+  DT_CHECK_ARG(groups <= 2048, "conv: %d (tap, channel chunk) groups per tile exceed the schedule table", groups);
+  Cfg::split(groups, NMMA, p.nrbuf > 0, p.split_out != 0, p.out_f32 != 0, &q.nstages, &q.ks, &q.ncbuf, &q.nrbuf);
+  q.ktab = (groups + 2) & ~1;
+  const int smem = Cfg::smem_bytes(groups, NMMA, q.nstages, q.ks, q.ncbuf, q.nrbuf, p.split_out != 0);
   DT_CHECK_ARG(q.nstages >= 2 && smem <= Cfg::BUDGET, "conv: smem split failed (%d stages, %d B)", q.nstages, smem);
   // DT_PDL=1 in the environment launches with programmatic stream serialization (the kernel waits on griddepcontrol
   // before its first global access).  Plain stream order is the default: inside the captured CUDA graph of a step
@@ -595,24 +624,27 @@ static int launch_conv1(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = at; lc.numAttrs = pdl ? 1 : 0;
-  DT_CHECK_CUDA(cudaLaunchKernelEx(&lc, conv_tc_kernel<BN, KIND, SPLIT>, tmA, tmB, tmC, tmR, q));
+  DT_CHECK_CUDA(cudaLaunchKernelEx(&lc, conv_tc_kernel<BN, KIND, SPLIT, NMMA>, tmA, tmB, tmC, tmR, q));
   return 0;
 }
 
-template <int BN, int KIND>
+template <int BN, int KIND, int NMMA>
 static int launch_conv2(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
                         const ConvKernelParams& p, int grid, cudaStream_t stream) {
-  return p.split_out ? launch_conv1<BN, KIND, true>(tmA, tmB, tmC, tmR, p, grid, stream)
-                     : launch_conv1<BN, KIND, false>(tmA, tmB, tmC, tmR, p, grid, stream);
+  return p.split_out ? launch_conv1<BN, KIND, true, NMMA>(tmA, tmB, tmC, tmR, p, grid, stream)
+                     : launch_conv1<BN, KIND, false, NMMA>(tmA, tmB, tmC, tmR, p, grid, stream);
 }
 
-// operand kind from the descriptor: tf32, else ab_format (1 bf16, 0 fp16)
+// operand kind from the descriptor: tf32, else ab_format (1 bf16, 0 fp16); split operands (bf16 or tf32 pairs) take
+// three MMA k-blocks per group
 template <int BN>
 static int launch_conv(bool tf32, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
                        const ConvKernelParams& p, int grid, cudaStream_t stream) {
-  if (tf32) return launch_conv2<BN, 2>(tmA, tmB, tmC, tmR, p, grid, stream);
-  return p.ab_format == 0 ? launch_conv2<BN, 1>(tmA, tmB, tmC, tmR, p, grid, stream)
-                          : launch_conv2<BN, 0>(tmA, tmB, tmC, tmR, p, grid, stream);
+  if (p.split_in) return tf32 ? launch_conv2<BN, 2, 3>(tmA, tmB, tmC, tmR, p, grid, stream)
+                              : launch_conv2<BN, 0, 3>(tmA, tmB, tmC, tmR, p, grid, stream);
+  if (tf32) return launch_conv2<BN, 2, 1>(tmA, tmB, tmC, tmR, p, grid, stream);
+  return p.ab_format == 0 ? launch_conv2<BN, 1, 1>(tmA, tmB, tmC, tmR, p, grid, stream)
+                          : launch_conv2<BN, 0, 1>(tmA, tmB, tmC, tmR, p, grid, stream);
 }
 
 }  // namespace dt
@@ -679,7 +711,6 @@ extern "C" int dt_conv3d(const dt_conv_desc* d, const void* x, const void* w, co
   // 3xTF32 split operands / outputs
   p.split_in = (d->x3 & 1) ? 1 : 0;
   p.split_out = (d->x3 & 2) ? 1 : 0;
-  p.nsub = p.split_in ? 3 : 1;
   p.ab_format = f16 ? 0 : 1;
   DT_CHECK_ARG(!p.split_in || d->Cin % BK == 0, "dt_conv3d: x3 inputs need Cin %% %d == 0 (Cin=%d)", BK, d->Cin);
   DT_CHECK_ARG(!p.split_out || ((tf32 ? out_f32 : !out_f32) && d->Cout % (out_f32 ? 32 : 64) == 0),
@@ -767,10 +798,11 @@ extern "C" int dt_conv3d(const dt_conv_desc* d, const void* x, const void* w, co
 // Planning query: MIRRORS the choices of dt_conv3d above (tile picker, column tile, residual ring, smem split) without
 // touching the device, so that the host logic is testable without a GPU (tests/test_conv_plan.py).
 template <int BN>
-static void plan_split(int kiters, bool res_tma, bool split_out, bool out_f32, dt_conv_plan_t* o) {
+static void plan_split(int groups, int nmma, bool res_tma, bool split_out, bool out_f32, dt_conv_plan_t* o) {
   using Cfg = ConvCfg<BN>;
-  Cfg::split(kiters, res_tma, split_out, out_f32, &o->stages, &o->ks, &o->ncbuf, &o->nrbuf);
-  o->smem_bytes = Cfg::smem_bytes(kiters, o->stages, o->ks, o->ncbuf, o->nrbuf, split_out);
+  Cfg::split(groups, nmma, res_tma, split_out, out_f32, &o->stages, &o->ks, &o->ncbuf, &o->nrbuf);
+  o->smem_bytes = Cfg::smem_bytes(groups, nmma, o->stages, o->ks, o->ncbuf, o->nrbuf, split_out);
+  o->stage_bytes = o->ks * Cfg::group_bytes(nmma);
 }
 
 extern "C" int dt_conv_plan(const dt_conv_desc* d, int residual_aligned, dt_conv_plan_t* o) {
@@ -795,14 +827,16 @@ extern "C" int dt_conv_plan(const dt_conv_desc* d, int residual_aligned, dt_conv
   const bool split_in = (d->x3 & 1) != 0, split_out = (d->x3 & 2) != 0;
   memset(o, 0, sizeof(*o));
   o->BN = BN; o->TH = ts.th; o->TW = ts.tw; o->TT = ts.tt; o->TB = ts.tb;
-  o->kiters = d->kT * d->kH * d->kW * cdiv(d->Cin, BK) * (split_in ? 3 : 1);
+  const int groups = d->kT * d->kH * d->kW * cdiv(d->Cin, BK);
+  const int nmma = split_in ? 3 : 1;
+  o->kiters = groups * nmma;
   const long long mt = (long long)cdiv(Wo, ts.tw) * cdiv(Ho, ts.th) * cdiv(To, ts.tt) * cdiv(d->N, ts.tb);
   o->tiles = (int)(mt * cdiv(d->Cout, BN));
   o->useful_rows = (double)Ho * Wo * To * d->N / ((double)mt * 128.0);
   switch (BN) {
-    case 128: plan_split<128>(o->kiters, res_tma, split_out, d->out_f32 != 0, o); break;
-    case 64: plan_split<64>(o->kiters, res_tma, split_out, d->out_f32 != 0, o); break;
-    default: plan_split<32>(o->kiters, res_tma, split_out, d->out_f32 != 0, o); break;
+    case 128: plan_split<128>(groups, nmma, res_tma, split_out, d->out_f32 != 0, o); break;
+    case 64: plan_split<64>(groups, nmma, res_tma, split_out, d->out_f32 != 0, o); break;
+    default: plan_split<32>(groups, nmma, res_tma, split_out, d->out_f32 != 0, o); break;
   }
   return 0;
 }
@@ -848,7 +882,7 @@ extern "C" int dt_conv1_7x7s2(const void* x_padded, int F, int Hp, int Wp, int C
   p.row_planes = 1;
   p.kchunks = 1;
   p.ab_format = 1;
-  p.nsub = x3 ? 2 : 1;
+  p.b_lo_blk = 1;                                  // x3: weight blocks 2*kh and 2*kh + 1 against one activation box
   p.split_out = x3 ? 1 : 0;
   p.out_lo_off = out_ld / 2;
   p.TH = TH; p.TW = TW; p.TT = 1; p.TB = 1; p.tiles_h = cdiv(Ho, TH); p.tiles_w = cdiv(Wo, TW); p.tiles_t = 1; p.tiles_b = F;
@@ -884,5 +918,6 @@ extern "C" int dt_conv1_7x7s2(const void* x_padded, int F, int Hp, int Wp, int C
   DT_CHECK_CUDA(cudaGetDevice(&dev));
   DT_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
-  return launch_conv<64>(tf32, tmA, tmB, tmC, tmC, p, grid, stream);
+  return x3 ? launch_conv1<64, 0, true, 2>(tmA, tmB, tmC, tmC, p, grid, stream)
+            : launch_conv<64>(tf32, tmA, tmB, tmC, tmC, p, grid, stream);
 }

@@ -180,13 +180,16 @@ int dt_conv3d(const dt_conv_desc* desc /*host*/, const void* x, const void* w, c
 
 /* Host-only planning query (no device work, usable without a GPU): the tiling dt_conv3d would pick for `desc` —
  * column tile BN, M tile (TB images x TT frames x TH x TW positions <= 128 rows), tiles per launch, operand ring
- * (stages x ks k-blocks), output staging / residual ring chunks, dynamic shared memory, k-blocks per tile and the
- * fraction of MMA rows that are real output positions.  residual_aligned: the residual pointer would be 16-byte
- * aligned (enables the TMA residual ring for bf16 residual modes). */
+ * (stages x ks (tap, channel chunk) groups of stage_bytes / ks bytes: one activation and one weight box, or with x3
+ * inputs the hi and lo box of each), output staging / residual ring chunks, dynamic shared memory, MMA k-blocks per
+ * tile (three per group with x3 inputs) and the fraction of MMA rows that are real output positions.
+ * residual_aligned: the residual pointer would be 16-byte aligned (enables the TMA residual ring for bf16 residual
+ * modes). */
 typedef struct dt_conv_plan_t {
   int BN, TH, TW, TT, TB;
   int tiles, kiters, stages, ks, ncbuf, nrbuf, smem_bytes;
   double useful_rows;
+  int stage_bytes;
 } dt_conv_plan_t;
 int dt_conv_plan(const dt_conv_desc* desc /*host*/, int residual_aligned, dt_conv_plan_t* plan /*host out*/);
 
