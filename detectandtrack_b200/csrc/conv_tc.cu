@@ -600,6 +600,49 @@ static int encode_out_map(CUtensorMap* m, void* y, int out_f32, int Cout, int Wo
   return encode_map(m, out_f32 != 0 ? 1 : 0, 5, y, d, st, b, e);
 }
 
+// What a descriptor launches, derived in one place for dt_conv3d and dt_conv_plan (the plan is what runs).
+// The descriptor's dtype and shape must have been validated by the caller.
+struct ConvGeom {
+  int To_full, To, Ho, Wo;
+  bool tf32, pointwise;
+  int BK;                      // elements per 128-byte k-block
+  TileShape ts;
+  int BN;                      // column tile
+  bool split_in, split_out;
+  int kchunks, groups, nmma;   // (tap, channel chunk) groups per tile, MMA k-blocks per group
+  bool res_tma;                // bf16 residual chunks arrive through the TMA ring
+  bool res_up;                 // ... as the (TH/2 x TW/2) box of the coarser map of the FPN top-down add
+};
+static ConvGeom conv_geom(const dt_conv_desc* d, bool residual_aligned) {
+  ConvGeom g;
+  g.tf32 = d->dtype == DT_DTYPE_TF32;
+  g.BK = g.tf32 ? 32 : 64;
+  g.To_full = (d->Ti + 2 * d->pT - d->kT) / d->sT + 1;
+  g.To = d->out_t_count > 0 ? d->out_t_count : g.To_full;
+  g.Ho = (d->Hi + 2 * d->pH - d->kH) / d->sH + 1;
+  g.Wo = (d->Wi + 2 * d->pW - d->kW) / d->sW + 1;
+  // stacking frames inside one TMA box needs unit temporal stride (pointwise convs fold strides into the map)
+  g.pointwise = d->kT == 1 && d->kH == 1 && d->kW == 1 && d->pT == 0 && d->pH == 0 && d->pW == 0;
+  g.ts = pick_tile(g.Ho, g.Wo, g.To, d->N, g.pointwise ? 256 : 256 / d->sW, g.pointwise ? 256 : 256 / d->sH,
+                   g.pointwise || d->sT == 1);
+  // each consumer warpgroup keeps a 64 x BN fp32 accumulator in registers: BN / 2 per thread, so 128 is the widest
+  // column tile that leaves the epilogue room under the 168-register cap of a 384-thread CTA
+  g.BN = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : 32);
+  g.split_in = (d->x3 & 1) != 0;
+  g.split_out = (d->x3 & 2) != 0;
+  g.kchunks = cdiv(d->Cin, g.BK);
+  g.groups = d->kT * d->kH * d->kW * g.kchunks;
+  g.nmma = g.split_in ? 3 : 1;                         // launch_conv: split operands take three products per group
+  // bf16 same-shape residual: its chunks are prefetched by TMA into a shared-memory ring (coalesced 128-byte
+  // rows instead of 4-byte global loads per thread pair).
+  // The FPN top-down add (res_mode 2) goes the same way when the tile is even-sized (tile origins are then even
+  // too): the (TH/2 x TW/2) box of the coarser map is loaded and each row serves its four children.
+  const bool res_even = (g.ts.th % 2 == 0) && (g.ts.tw % 2 == 0);
+  g.res_tma = (d->res_mode == 1 || (d->res_mode == 2 && res_even)) && !d->out_f32 && !g.tf32 && residual_aligned;
+  g.res_up = g.res_tma && d->res_mode == 2;
+  return g;
+}
+
 template <int BN, int KIND, bool SPLIT, int NMMA>
 static int launch_conv1(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
                        const ConvKernelParams& p, int grid, cudaStream_t stream) {
@@ -656,23 +699,22 @@ extern "C" int dt_conv3d(const dt_conv_desc* d, const void* x, const void* w, co
   cudaStream_t stream = (cudaStream_t)stream_;
   DT_CHECK_ARG(d != nullptr, "dt_conv3d: null descriptor");
   DT_CHECK_ARG(d->dtype == DT_DTYPE_BF16 || d->dtype == DT_DTYPE_TF32 || d->dtype == DT_DTYPE_F16, "dt_conv3d: dtype %d not in {BF16, TF32, F16}", d->dtype);
-  const bool tf32 = d->dtype == DT_DTYPE_TF32;
   const bool f16 = d->dtype == DT_DTYPE_F16;          // fp16 x and w (11-bit operands, one MMA per product); outputs stay bf16 / fp32
   DT_CHECK_ARG(!f16 || (!(d->x3 & 1) && d->res_mode == 0), "dt_conv3d: DT_DTYPE_F16 inputs are plain rows and take no residual");
-  const int in_dt = tf32 ? 1 : (f16 ? 2 : 0);
-  const int esz = tf32 ? 4 : 2;
-  const int BK = tf32 ? 32 : 64;
   DT_CHECK_ARG(d->N >= 1 && d->Ti >= 1 && d->Hi >= 1 && d->Wi >= 1 && d->Cin >= 1 && d->Cout >= 1,
                "dt_conv3d: bad input shape N=%d T=%d H=%d W=%d Cin=%d Cout=%d", d->N, d->Ti, d->Hi, d->Wi, d->Cin, d->Cout);
   DT_CHECK_ARG(d->kT >= 1 && d->kH >= 1 && d->kW >= 1 && d->sT >= 1 && d->sH >= 1 && d->sW >= 1 && d->pT >= 0 &&
                    d->pH >= 0 && d->pW >= 0, "dt_conv3d: bad filter geometry");
-  const int To_full = (d->Ti + 2 * d->pT - d->kT) / d->sT + 1;
+  const ConvGeom g = conv_geom(d, ((uintptr_t)residual % 16) == 0);
+  const bool tf32 = g.tf32;
+  const int in_dt = tf32 ? 1 : (f16 ? 2 : 0);
+  const int esz = tf32 ? 4 : 2;
+  const int BK = g.BK;
+  const int To_full = g.To_full;
   DT_CHECK_ARG(d->out_t_first >= 0 && d->out_t_count >= 0 && d->out_t_first + d->out_t_count <= (To_full > 0 ? To_full : 0),
                "dt_conv3d: output frame range [%d, +%d) outside the %d output frames", d->out_t_first, d->out_t_count, To_full);
   DT_CHECK_ARG(d->out_t_count == 0 || d->res_mode == 0, "dt_conv3d: an output frame range cannot be combined with a residual");
-  const int To = d->out_t_count > 0 ? d->out_t_count : To_full;
-  const int Ho = (d->Hi + 2 * d->pH - d->kH) / d->sH + 1;
-  const int Wo = (d->Wi + 2 * d->pW - d->kW) / d->sW + 1;
+  const int To = g.To, Ho = g.Ho, Wo = g.Wo;
   DT_CHECK_ARG(To >= 1 && Ho >= 1 && Wo >= 1, "dt_conv3d: empty output (%d,%d,%d)", To, Ho, Wo);
   const int in_ld = d->in_ld > 0 ? d->in_ld : d->Cin;
   const int w_ld = d->w_ld > 0 ? d->w_ld : d->Cin;
@@ -692,25 +734,23 @@ extern "C" int dt_conv3d(const dt_conv_desc* d, const void* x, const void* w, co
   DT_CHECK_ARG((out_ld * oesz) % 16 == 0 && (d->res_mode == 0 || (res_ld * oesz) % 16 == 0),
                "dt_conv3d: out_ld/res_ld rows must be 16-byte multiples");
 
-  // stacking frames inside one TMA box needs unit temporal stride (pointwise convs fold strides into the map)
-  const bool pointwise = d->kT == 1 && d->kH == 1 && d->kW == 1 && d->pT == 0 && d->pH == 0 && d->pW == 0;
-  const TileShape ts = pick_tile(Ho, Wo, To, d->N, pointwise ? 256 : 256 / d->sW, pointwise ? 256 : 256 / d->sH,
-                                 pointwise || d->sT == 1);
+  const bool pointwise = g.pointwise;
+  const TileShape ts = g.ts;
   const int TH = ts.th, TW = ts.tw;
   ConvKernelParams p;
   memset(&p, 0, sizeof(p));
   p.N = d->N; p.To = To; p.Ho = Ho; p.Wo = Wo; p.Cout = d->Cout;
   p.kT = d->kT; p.kH = d->kH; p.kW = d->kW; p.pT = d->pT; p.pH = d->pH; p.pW = d->pW;
   p.sT = d->sT; p.sH = d->sH; p.sW = d->sW;
-  p.kchunks = cdiv(d->Cin, BK);
+  p.kchunks = g.kchunks;
   p.TH = TH; p.TW = TW; p.TT = ts.tt; p.TB = ts.tb;
   p.tiles_h = cdiv(Ho, TH); p.tiles_w = cdiv(Wo, TW); p.tiles_t = cdiv(To, ts.tt); p.tiles_b = cdiv(d->N, ts.tb);
   p.a_bytes = (uint32_t)(TH * TW * ts.tt * ts.tb) * 128u;
   p.scale = scale; p.bias = bias; p.residual = residual; p.res_mode = d->res_mode; p.res_ld = res_ld;
   p.relu = d->relu; p.out_f32 = out_f32; p.round_tf32 = d->out_round_tf32;
   // 3xTF32 split operands / outputs
-  p.split_in = (d->x3 & 1) ? 1 : 0;
-  p.split_out = (d->x3 & 2) ? 1 : 0;
+  p.split_in = g.split_in ? 1 : 0;
+  p.split_out = g.split_out ? 1 : 0;
   p.ab_format = f16 ? 0 : 1;
   DT_CHECK_ARG(!p.split_in || d->Cin % BK == 0, "dt_conv3d: x3 inputs need Cin %% %d == 0 (Cin=%d)", BK, d->Cin);
   DT_CHECK_ARG(!p.split_out || ((tf32 ? out_f32 : !out_f32) && d->Cout % (out_f32 ? 32 : 64) == 0),
@@ -722,19 +762,11 @@ extern "C" int dt_conv3d(const dt_conv_desc* d, const void* x, const void* w, co
   DT_CHECK_ARG(!p.split_in || (p.a_lo_off + d->Cin <= in_ld && p.b_lo_off >= d->Cin), "dt_conv3d: x3 lo halves do not fit the rows");
   DT_CHECK_ARG(!p.split_out || p.out_lo_off + d->Cout <= out_ld, "dt_conv3d: x3 output lo half does not fit the row");
 
-  // each consumer warpgroup keeps a 64 x BN fp32 accumulator in registers: BN / 2 per thread, so 128 is the widest
-  // column tile that leaves the epilogue room under the 168-register cap of a 384-thread CTA
-  const int BN = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : 32);
-  // bf16 same-shape residual: its chunks are prefetched by TMA into a shared-memory ring (coalesced 128-byte
-  // rows instead of 4-byte global loads per thread pair).
-  // The FPN top-down add (res_mode 2) goes the same way when the tile is even-sized (tile origins are then even
-  // too): the (TH/2 x TW/2) box of the coarser map is loaded and each row serves its four children.
-  const bool res_even = (TH % 2 == 0) && (TW % 2 == 0);
-  const bool res_tma = (d->res_mode == 1 || (d->res_mode == 2 && res_even)) && !out_f32 && !tf32 &&
-                       ((uintptr_t)residual % 16) == 0;
+  const int BN = g.BN;
+  const bool res_tma = g.res_tma;
   p.t_first = d->out_t_count > 0 ? d->out_t_first : 0;
   p.nrbuf = res_tma ? 1 : 0;                         // ring depth is chosen with the smem split at launch
-  p.res_up = (res_tma && d->res_mode == 2) ? 1 : 0;
+  p.res_up = g.res_up ? 1 : 0;
   p.tiles_n = cdiv(d->Cout, BN);
   p.fd_n = make_fastdiv(p.tiles_n); p.fd_w = make_fastdiv(p.tiles_w); p.fd_h = make_fastdiv(p.tiles_h); p.fd_t = make_fastdiv(p.tiles_t);
   const long long total = (long long)p.tiles_b * p.tiles_t * p.tiles_h * p.tiles_w * p.tiles_n;
@@ -795,8 +827,8 @@ extern "C" int dt_conv3d(const dt_conv_desc* d, const void* x, const void* w, co
 }
 
 
-// Planning query: MIRRORS the choices of dt_conv3d above (tile picker, column tile, residual ring, smem split) without
-// touching the device, so that the host logic is testable without a GPU (tests/test_conv_plan.py).
+// Planning query: the choices of dt_conv3d above (conv_geom, then the smem split of launch_conv1) without touching the
+// device, so that the host logic is testable without a GPU (tests/test_conv_plan.py).
 template <int BN>
 static void plan_split(int groups, int nmma, bool res_tma, bool split_out, bool out_f32, dt_conv_plan_t* o) {
   using Cfg = ConvCfg<BN>;
@@ -807,36 +839,24 @@ static void plan_split(int groups, int nmma, bool res_tma, bool split_out, bool 
 
 extern "C" int dt_conv_plan(const dt_conv_desc* d, int residual_aligned, dt_conv_plan_t* o) {
   DT_CHECK_ARG(d != nullptr && o != nullptr, "dt_conv_plan: null pointer");
-  DT_CHECK_ARG(d->dtype == DT_DTYPE_BF16 || d->dtype == DT_DTYPE_TF32, "dt_conv_plan: dtype %d not in {BF16, TF32}", d->dtype);
+  DT_CHECK_ARG(d->dtype == DT_DTYPE_BF16 || d->dtype == DT_DTYPE_TF32 || d->dtype == DT_DTYPE_F16,
+               "dt_conv_plan: dtype %d not in {BF16, TF32, F16}", d->dtype);
   DT_CHECK_ARG(d->N >= 1 && d->Ti >= 1 && d->Hi >= 1 && d->Wi >= 1 && d->Cin >= 1 && d->Cout >= 1 && d->kT >= 1 && d->kH >= 1 &&
                    d->kW >= 1 && d->sT >= 1 && d->sH >= 1 && d->sW >= 1 && d->pT >= 0 && d->pH >= 0 && d->pW >= 0,
                "dt_conv_plan: bad shape");
-  const bool tf32 = d->dtype == DT_DTYPE_TF32;
-  const int BK = tf32 ? 32 : 64;
-  const int To_full = (d->Ti + 2 * d->pT - d->kT) / d->sT + 1;
-  const int To = d->out_t_count > 0 ? d->out_t_count : To_full;
-  const int Ho = (d->Hi + 2 * d->pH - d->kH) / d->sH + 1;
-  const int Wo = (d->Wi + 2 * d->pW - d->kW) / d->sW + 1;
-  DT_CHECK_ARG(To >= 1 && Ho >= 1 && Wo >= 1, "dt_conv_plan: empty output (%d,%d,%d)", To, Ho, Wo);
-  const bool pointwise = d->kT == 1 && d->kH == 1 && d->kW == 1 && d->pT == 0 && d->pH == 0 && d->pW == 0;
-  const TileShape ts = pick_tile(Ho, Wo, To, d->N, pointwise ? 256 : 256 / d->sW, pointwise ? 256 : 256 / d->sH,
-                                 pointwise || d->sT == 1);
-  const int BN = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : 32);
-  const bool res_even = (ts.th % 2 == 0) && (ts.tw % 2 == 0);
-  const bool res_tma = (d->res_mode == 1 || (d->res_mode == 2 && res_even)) && !d->out_f32 && !tf32 && residual_aligned;
-  const bool split_in = (d->x3 & 1) != 0, split_out = (d->x3 & 2) != 0;
+  const ConvGeom g = conv_geom(d, residual_aligned != 0);
+  DT_CHECK_ARG(g.To >= 1 && g.Ho >= 1 && g.Wo >= 1, "dt_conv_plan: empty output (%d,%d,%d)", g.To, g.Ho, g.Wo);
+  const TileShape ts = g.ts;
   memset(o, 0, sizeof(*o));
-  o->BN = BN; o->TH = ts.th; o->TW = ts.tw; o->TT = ts.tt; o->TB = ts.tb;
-  const int groups = d->kT * d->kH * d->kW * cdiv(d->Cin, BK);
-  const int nmma = split_in ? 3 : 1;
-  o->kiters = groups * nmma;
-  const long long mt = (long long)cdiv(Wo, ts.tw) * cdiv(Ho, ts.th) * cdiv(To, ts.tt) * cdiv(d->N, ts.tb);
-  o->tiles = (int)(mt * cdiv(d->Cout, BN));
-  o->useful_rows = (double)Ho * Wo * To * d->N / ((double)mt * 128.0);
-  switch (BN) {
-    case 128: plan_split<128>(groups, nmma, res_tma, split_out, d->out_f32 != 0, o); break;
-    case 64: plan_split<64>(groups, nmma, res_tma, split_out, d->out_f32 != 0, o); break;
-    default: plan_split<32>(groups, nmma, res_tma, split_out, d->out_f32 != 0, o); break;
+  o->BN = g.BN; o->TH = ts.th; o->TW = ts.tw; o->TT = ts.tt; o->TB = ts.tb;
+  o->kiters = g.groups * g.nmma;
+  const long long mt = (long long)cdiv(g.Wo, ts.tw) * cdiv(g.Ho, ts.th) * cdiv(g.To, ts.tt) * cdiv(d->N, ts.tb);
+  o->tiles = (int)(mt * cdiv(d->Cout, g.BN));
+  o->useful_rows = (double)g.Ho * g.Wo * g.To * d->N / ((double)mt * 128.0);
+  switch (g.BN) {
+    case 128: plan_split<128>(g.groups, g.nmma, g.res_tma, g.split_out, d->out_f32 != 0, o); break;
+    case 64: plan_split<64>(g.groups, g.nmma, g.res_tma, g.split_out, d->out_f32 != 0, o); break;
+    default: plan_split<32>(g.groups, g.nmma, g.res_tma, g.split_out, d->out_f32 != 0, o); break;
   }
   return 0;
 }

@@ -36,6 +36,13 @@ def _ref_conv(x, w, stride, pad, scale, bias, residual, res_mode, relu):
     return y.float()
 
 
+def _within_bf16_output(y, ref):
+    """bf16 outputs: |y - ref| <= 2^-8 |ref| + 2e-4 max|ref| elementwise, half a bf16 ulp of output rounding plus the
+    fp32 accumulation-order error."""
+    y, ref = y.double(), ref.double()
+    return bool(((y - ref).abs() <= 2 ** -8 * ref.abs() + 2e-4 * ref.abs().max()).all())
+
+
 CASES = [
     # N, T, H, W, Cin, Cout, k, stride, pad, affine, res_mode, relu
     dict(N=1, T=1, H=16, W=16, Cin=64, Cout=64, k=(1, 1, 1), s=(1, 1, 1), p=(0, 0, 0)),
@@ -144,7 +151,7 @@ def test_conv_bf16_output_and_channel_slices():
     ref = _ref_conv(x[..., :64].float(), w.float(), (1, 1, 1), (0, 1, 1), None, None, None, 0, True)
     got = out.cpu().float()
     assert torch.all(got[..., 64:] == 0)
-    assert (got[..., :64] - ref).abs().max().item() <= 1e-2 * ref.abs().max().item()     # bf16 output rounding (2^-8)
+    assert _within_bf16_output(got[..., :64], ref)
 
 
 @pytest.mark.parametrize('shape', [(1, 3, 40, 56, 64, 256), (11, 1, 14, 14, 128, 200), (2, 3, 25, 42, 64, 256), (2, 1, 16, 32, 64, 256),
@@ -171,7 +178,7 @@ def test_conv_bf16_residual_epilogue(shape, res_mode):
     torch.cuda.synchronize()
     ref = _ref_conv(x.float(), w.float(), (1, 1, 1), (0, 0, 0), scale, bias, res.float(), res_mode, True)
     assert y.dtype == torch.bfloat16 and y.shape == ref.shape
-    assert (y.cpu().float() - ref).abs().max().item() <= 1e-2 * ref.abs().max().item()   # bf16 output rounding (2^-8)
+    assert _within_bf16_output(y.cpu().float(), ref)
 
 
 def test_conv_time_major_output():
@@ -219,11 +226,23 @@ def test_conv_rejects_bad_arguments():
 @pytest.mark.parametrize('mode', ['bf16', 'tf32', 'bf16x3'])
 def test_conv1_packed_rows_vs_torch(mode):
     """dt_conv1_7x7s2 (filter row packed into K over a zero-bordered blob) == conv 7x7 s2 p3 + affine + relu."""
+    _check_conv1_packed_rows(mode, 3, 64, 96)
+
+
+@pytest.mark.parametrize('mode', ['bf16', 'tf32', 'bf16x3'])
+def test_conv1_packed_rows_three_tiles_per_cta(mode):
+    """The same at three 256 x 336 frames: every CTA walks at least three 128-row tiles."""
+    import torch
+    Fr, H, W = 3, 256, 336
+    assert Fr * (H // 2) * (W // 2) / 128 >= 3 * torch.cuda.get_device_properties(0).multi_processor_count
+    _check_conv1_packed_rows(mode, Fr, H, W)
+
+
+def _check_conv1_packed_rows(mode, Fr, H, W):
     import torch
     import torch.nn.functional as F
     from detectandtrack_b200.ops import conv as cv, dense_ops
     g = torch.Generator().manual_seed(11)
-    Fr, H, W = 3, 64, 96
     frames = torch.randint(0, 256, (Fr, H, W, 3), generator=g, dtype=torch.uint8)
     means = (102.9801, 115.9465, 122.7717)
     w = torch.randn((64, 3, 1, 7, 7), generator=g) * 0.01
@@ -252,3 +271,246 @@ def test_conv1_packed_rows_vs_torch(mode):
     tol = 2e-4 if mode == 'bf16' else 1.5e-3
     assert y.shape == ref.shape
     assert (y - ref).abs().max().item() <= tol * ref.abs().max().item()
+    if mode == 'bf16':
+        # the engine's bf16 conv1 writes bf16: half a bf16 ulp of rounding on top of the accumulation-order error
+        yb = cv.conv1_7x7s2(x, wp, (H, W), sc.cuda(), bi.cuda(), relu=True, dtype=dtype).cpu()
+        assert _within_bf16_output(yb, ref)
+
+
+def test_conv1_exact_fp32_vs_fp64():
+    """dt_conv1_7x7s2_f32 (the tf32x3 mode's conv1) is plain fp32: each output is within the fp32 rounding bound of a
+    147-term sum, sum_k |x_k w_k| * 147 * 2^-24, plus the affine rounding and the tf32 pair storage (2^-22) of the
+    value, against an fp64 conv of the same fp32 blob.  Three 256 x 336 frames: many CTAs of 32 pixels each."""
+    import torch
+    import torch.nn.functional as F
+    from detectandtrack_b200.ops import conv as cv, dense_ops
+    g = torch.Generator().manual_seed(12)
+    Fr, H, W = 3, 256, 336
+    frames = torch.randint(0, 256, (Fr, H, W, 3), generator=g, dtype=torch.uint8)
+    blob = dense_ops.prep_clip(frames.cuda(), (102.9801, 115.9465, 122.7717), 1.0, (H, W), (H, W), cpad=4, out_f32=2)
+    w = torch.randn((64, 3, 7, 7), generator=g) * 0.01
+    sc = torch.rand(64, generator=g) + 0.5
+    bi = torch.randn(64, generator=g) * 0.1
+    y = cv.join_tf32(cv.conv1_7x7s2_f32(blob, cv.pack_conv1_weight_f32(w), sc.cuda(), bi.cuda())).cpu().double()
+    xin = blob[..., :3].cpu().double().permute(0, 3, 1, 2)
+    s4, b4 = sc.double().view(1, -1, 1, 1), bi.double().view(1, -1, 1, 1)
+    ref = (F.conv2d(xin, w.double(), None, 2, 3) * s4 + b4).clamp_min(0).permute(0, 2, 3, 1)
+    mag = (F.conv2d(xin.abs(), w.double().abs(), None, 2, 3) * s4.abs()).permute(0, 2, 3, 1)
+    bound = 2 ** -24 * (147 * mag + 5 * ref.abs()) + 1e-30
+    assert y.shape == ref.shape
+    ratio = ((y - ref).abs() / bound).max().item()
+    assert ratio <= 1.0, ratio
+
+
+def test_pairs_to_f16_rounds_and_saturates_like_torch():
+    """dt_pairs_to_f16 == fp16(clamp(hi + lo, +-65504)) bit for bit, from fp16 subnormals to values beyond its range."""
+    import torch
+    from detectandtrack_b200.ops import conv as cv, dense_ops
+    g = torch.Generator().manual_seed(13)
+    v = torch.randn((777, 256), generator=g) * 10.0 ** (torch.rand((777, 256), generator=g) * 14 - 8)
+    v[0, :8] = torch.tensor([65504., 65519., 65520., 1e5, -65504., -65520., -3e38, 3e38])
+    pairs = cv.split_bf16(v.cuda())
+    got = dense_ops.pairs_to_f16(pairs).cpu()
+    hi, lo = pairs[..., :256].float().cpu(), pairs[..., 256:].float().cpu()
+    want = (hi + lo).clamp(-65504, 65504).half()
+    assert (want.abs() == 65504).sum() > 8 and torch.isfinite(got).all()
+    assert torch.equal(got.view(torch.int16), want.view(torch.int16))
+
+
+# ------------------------------------------------------------------ every conv plan of the benchmarked step, multi-tile
+from test_conv_plan import R50_FPN_3D, REDUCED, conv_args, layer_modes, step_plan  # noqa: E402
+from test_conv_reference import conv_ref  # noqa: E402
+
+STEP_CASES = [(l, m) for l in R50_FPN_3D for m in layer_modes(l)]
+# DESIGN.md §4, max-norm.  bf16 / f16: the reference gets the same rounded operands, so only the fp32 accumulation order
+# differs; bf16 outputs are checked elementwise instead (below).
+STEP_TOL = {'bf16': 2e-4, 'f16': 2e-4, 'tf32': 1e-3, 'tf32x3': 1e-4, 'bf16x3': 1e-4}
+
+
+def _step_tol(layer, mode):
+    """STEP_TOL, except tf32x3 beyond K = 8192 products per output: there the bound grows in proportion to K.  The
+    tensor cores do not round to nearest when they add into the fp32 accumulator, so the error is biased and grows
+    linearly with the wgmma steps per output rather than with their square root.  tf32x3 takes the most steps (8
+    products per step, three products per pair): on an H100 its worst error was 0.51e-4 of max|ref| at K = 6912,
+    0.89e-4 at 12544 (fc6) and 1.03e-4 at 13824 (res5 3x3x3), and bf16x3 (16 products per step) exactly half of that."""
+    K = layer[5] * layer[7][0] * layer[7][1] * layer[7][2]
+    return STEP_TOL[mode] * (max(1.0, K / 8192) if mode == 'tf32x3' else 1.0)
+
+
+def _epilogue(name):
+    """(AffineChannel, ReLU) of a layer as the engine fuses it: the ResNet body convs carry a frozen-BN affine (no
+    ReLU on the projection shortcut); everything else a bias, ReLU on the RPN / keypoint convs and the FCs."""
+    if name.startswith('res'):
+        return True, 'branch1' not in name
+    return False, name.startswith(('rpn conv', 'fc6', 'keypoint head'))
+
+
+def _step_inputs(layer, mode, g):
+    """Device tensors of one layer at its reduced shape, stored the way the engine stores them in `mode`, and the
+    values the kernel reads from them (rounded operands, hi + lo pairs, the stored residual) for the reference."""
+    import torch
+    from detectandtrack_b200.ops import conv as cv, dense_ops
+    name, _, _, _, _, Cin, Cout, k, s, p, rm = layer
+    N, T, H, W = REDUCED[name]
+    To, Ho, Wo = (T + 2 * p[0] - k[0]) // s[0] + 1, (H + 2 * p[1] - k[1]) // s[1] + 1, (W + 2 * p[2] - k[2]) // s[2] + 1
+    dt = cv.F16 if mode == 'f16' else cv.MODE_NAMES[mode]
+    split = dt in cv.SPLIT_MODES
+    affine, relu = _epilogue(name)
+    x = torch.randn((N, T, H, W, Cin), generator=g, device='cuda')
+    w = torch.randn((Cout, Cin) + k, generator=g, device='cuda') * (2.0 / (Cin * k[0] * k[1] * k[2])) ** 0.5
+    scale = torch.rand(Cout, generator=g, device='cuda') + 0.5 if affine else None
+    bias = torch.randn(Cout, generator=g, device='cuda') * 0.1
+    res = None
+    if rm:
+        res = torch.randn((N, To, Ho // rm, Wo // rm, Cout), generator=g, device='cuda')
+    wp = cv.pack_weight(w, dt)
+    wr = (cv.join_split(wp) if split else wp.float())[:, :, :Cin]            # [taps, Cout, Cin] as the kernel reads it
+    wr = wr.reshape(k + (Cout, Cin)).permute(3, 4, 0, 1, 2)
+    if mode == 'f16':
+        xd = dense_ops.pairs_to_f16(cv.split_bf16(x))                          # the bf16x3h engine's post-hoc input
+    elif split:
+        xd = cv.split_for(dt, x)
+    else:
+        xd = {'bf16': x.bfloat16(), 'tf32': cv.round_tf32(x)}[mode]
+    xr = cv.join_split(xd) if split else xd.float()
+    if res is not None:
+        res = cv.split_for(dt, res) if split else (res.bfloat16() if mode == 'bf16' else res)
+    resr = None if res is None else (cv.join_split(res) if split else res.float())
+    head = Cout % 64 != 0
+    out = None
+    if head:                                       # final fp32 head outputs, in a row padded to 16 bytes as the engine does
+        out = torch.empty((N, To, Ho, Wo, (Cout + 3) // 4 * 4), dtype=torch.float32, device='cuda')
+    run = dict(x=xd, w=wp, k=k, s=s, p=p, scale=scale, bias=bias, res=res, rm=rm, relu=relu, dtype=dt, out=out,
+               out_f32=True if head else None, split_out=True if mode == 'f16' else None)
+    ref = dict(x=xr, w=wr, scale=scale, bias=bias, residual=resr, res_mode=rm, relu=relu)
+    return run, ref
+
+
+def _locate(idx, shape, o, sms):
+    """Output element (n, t, h, w, c) -> its (M tile, column tile), linear tile index, and the CTA that ran it."""
+    n, t, h, w, c = idx
+    _, To, Ho, Wo, Cout = shape
+    tw, th, tt = -(-Wo // o.TW), -(-Ho // o.TH), -(-To // o.TT)
+    tn = -(-Cout // o.BN)
+    m = ((n // o.TB * tt + t // o.TT) * th + h // o.TH) * tw + w // o.TW
+    tile = m * tn + c // o.BN
+    return ('M tile %d (image %d, frame %d, row %d, column %d tile), column tile %d: tile %d = tile %d of CTA %d'
+            % (m, n // o.TB, t // o.TT, h // o.TH, w // o.TW, c // o.BN, tile, tile // sms, tile % sms))
+
+
+@pytest.mark.parametrize('layer,mode', STEP_CASES, ids=['%s-%s' % (l[0], m) for l, m in STEP_CASES])
+def test_step_layer_over_three_waves_vs_fp64(layer, mode, record_property):
+    """Every (layer, mode) of the benchmarked step at its reduced shape (test_conv_plan.REDUCED: the step's plan, three
+    or more tiles per CTA, a ragged last wave) with the engine's storage and epilogue, against the fp64 tap-sum
+    reference on the values the kernel reads.  bf16 outputs: |y - ref| <= 2^-8 |ref| + 2e-4 max|ref| elementwise (half a
+    bf16 ulp of output rounding plus the accumulation-order error); the others _step_tol * max|ref|."""
+    import zlib
+    import torch
+    from detectandtrack_b200.ops import conv as cv
+    name, Cout = layer[0], layer[6]
+    o = step_plan(layer, mode, reduced=True)
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    assert o.tiles / sms >= 3, (name, mode, o.tiles, sms)
+    g = torch.Generator(device='cuda').manual_seed(zlib.crc32(('%s/%s' % (name, mode)).encode()))
+    run, ref_in = _step_inputs(layer, mode, g)
+    y = cv.conv3d(run['x'], run['w'], run['k'], run['s'], run['p'], run['scale'], run['bias'], run['res'], run['rm'],
+                  run['relu'], out_f32=run['out_f32'], dtype=run['dtype'], out=run['out'], split_out=run['split_out'])
+    if run['out'] is not None:
+        y = y[..., :Cout]
+    elif run['split_out'] or run['dtype'] in cv.SPLIT_MODES:
+        y = cv.join_split(y)
+    bf16_out = y.dtype == torch.bfloat16
+    ref = conv_ref(ref_in['x'], ref_in['w'], layer[8], layer[9], ref_in['scale'], ref_in['bias'], ref_in['residual'],
+                   ref_in['res_mode'], ref_in['relu'])
+    assert y.shape == ref.shape
+    err = (y.double() - ref).abs()
+    den = ref.abs().max().item()
+    bound = 2 ** -8 * ref.abs() + 2e-4 * den if bf16_out else _step_tol(layer, mode) * den
+    ratio = err / bound
+    worst = ratio.max().item()
+    record_property('tiles', o.tiles)
+    record_property('tiles_per_cta', round(o.tiles / sms, 2))
+    record_property('worst_err_over_tol', worst)
+    if not worst <= 1.0:                           # NaN too: a wrong shared-memory read can produce it
+        idx = [int(i) for i in torch.unravel_index(ratio.argmax(), ratio.shape)]
+        pytest.fail('%s %s: error %.3g x the bound at %s, %s' % (name, mode, worst, idx, _locate(idx, y.shape, o, sms)))
+
+
+@pytest.mark.parametrize('mode', ['bf16x3', 'f16'])
+def test_posthoc_fpn_time_major_and_center_frame_vs_fp64(mode):
+    """The post-hoc FPN conv as the slice-center link runs it: frames-outermost output (time_major) and the centre
+    output frame alone (out_frames=(1, 1)), in bf16x3 and with fp16 operands writing bf16 pairs (bf16x3h)."""
+    import torch
+    from detectandtrack_b200.ops import conv as cv
+    layer = next(l for l in R50_FPN_3D if l[0] == 'fpn post-hoc P4')
+    g = torch.Generator(device='cuda').manual_seed(14)
+    run, ref_in = _step_inputs(layer, mode, g)
+    ref = conv_ref(ref_in['x'], ref_in['w'], layer[8], layer[9], None, ref_in['bias'])
+    kw = dict(dtype=run['dtype'], split_out=run['split_out'])
+    tm = cv.conv3d(run['x'], run['w'], run['k'], run['s'], run['p'], None, run['bias'], time_major=True, **kw)
+    mid = cv.conv3d(run['x'], run['w'], run['k'], run['s'], run['p'], None, run['bias'], out_frames=(1, 1), **kw)
+    assert not tm.is_contiguous() and tm[:, 1:2].is_contiguous() and mid.shape[1] == 1
+    tol = STEP_TOL[mode] * ref.abs().max().item()
+    assert (cv.join_split(tm).double() - ref).abs().max().item() <= tol
+    assert (cv.join_split(mid).double() - ref[:, 1:2]).abs().max().item() <= tol
+
+
+def test_step_convs_are_all_in_the_table(monkeypatch, record_property):
+    """One 800 x 1333 clip of the benchmarked R50-FPN-3D config through DetectionEngine.detect in bf16, bf16x3,
+    bf16x3h and tf32x3: every conv_tc launch has a plan key (storage, residual kind, BN, schedule length, ring, staging
+    and residual split) of a test_conv_plan.R50_FPN_3D layer, which the value test above checks at three or more tiles
+    per CTA; every conv1 launch runs a variant test_conv1_packed_rows_vs_torch / test_conv1_exact_fp32_vs_fp64 check."""
+    import ctypes as C
+    import torch
+    import bench
+    from detectandtrack_b200 import _lib as L
+    from detectandtrack_b200.modeling import params as P
+    from detectandtrack_b200.modeling.engine import DetectionEngine
+    from detectandtrack_b200.ops import conv as cv
+    from test_conv_plan import plan_key, table_plan_keys
+    table = table_plan_keys()
+    conv1_tested = {('conv1', 0, 1, 0), ('conv1', 0, 0, 0), ('conv1', 1, 1, 0), ('conv1', 0, 0, 1), ('conv1_f32', 0)}
+    calls, launched = {'py': 0, 'c': 0}, []
+    orig_call = L.call
+
+    def spy(name, *a):
+        if name == 'dt_conv3d':
+            d = a[0]._obj
+            o = L.ConvPlan()
+            aligned = a[5] is None or a[5].value % 16 == 0
+            assert L.lib().dt_conv_plan(C.byref(d), int(aligned), C.byref(o)) == 0, L.lib().dt_last_error()
+            launched.append((plan_key(d.dtype, d.x3, d.out_f32, d.res_mode, o), (d.N, d.Ti, d.Hi, d.Wi, d.Cin, d.Cout)))
+        elif name == 'dt_conv1_7x7s2':
+            launched.append((('conv1', a[10], a[11], a[13]), None))
+        elif name == 'dt_conv1_7x7s2_f32':
+            launched.append((('conv1_f32', a[8]), None))
+        if name.startswith(('dt_conv3d', 'dt_conv1_7x7s2')):
+            calls['c'] += 1
+        return orig_call(name, *a)
+
+    def counted(f):
+        def wrapped(*a, **kw):
+            calls['py'] += 1
+            return f(*a, **kw)
+        return wrapped
+    monkeypatch.setattr(L, 'call', spy)
+    for f in ('conv3d', 'conv1_7x7s2', 'conv1_7x7s2_f32'):
+        monkeypatch.setattr(cv, f, counted(getattr(cv, f)))
+    cfg = bench.bench_cfg(800, 1333)
+    blobs, spec = P.random_blobs(cfg)
+    frames = torch.from_numpy(bench.synth_frames(1, bench.frames_per_clip(cfg), 800, 1333, 7)).cuda()
+    missing = {}
+    for mode in ('bf16', 'bf16x3', 'bf16x3h', 'tf32x3'):
+        del launched[:]
+        eng = DetectionEngine(cfg, blobs, spec, dtype=mode)
+        eng.detect(frames)
+        torch.cuda.synchronize()
+        assert len(launched) > 50
+        record_property('launches_' + mode, len(launched))
+        record_property('plan_keys_' + mode, len({k for k, _ in launched}))
+        for key, shape in launched:
+            if key not in table and key not in conv1_tested:
+                missing.setdefault(key, (mode, shape))
+        del eng
+    assert calls['py'] == calls['c']
+    assert not missing, missing
