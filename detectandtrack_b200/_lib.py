@@ -68,8 +68,9 @@ SIGNATURES = {
     'dt_sample_rois': [_p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p, _i, _i, _i, _p, _i, _i, _f, _f, _f, _f, C.POINTER(_f), _i,
                        C.c_ulonglong, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p, _p],
 }
-# host-only helpers (not error-code functions)
-HOST_FUNCS = {'dt_planes_ld': ([_i, _i, _i, _i], C.c_int), 'dt_jpeg_available': ([], C.c_int)}
+# host-only helpers: no device work, usable without a GPU (dt_wgrad_nhwc_plan returns 0 or an error code like the rest)
+HOST_FUNCS = {'dt_planes_ld': ([_i, _i, _i, _i], C.c_int), 'dt_jpeg_available': ([], C.c_int),
+              'dt_wgrad_nhwc_plan': ([_i] * 15 + [C.c_void_p], C.c_int)}
 
 
 
@@ -105,6 +106,12 @@ class ConvPlan(C.Structure):
     """dt_conv_plan_t (include/dt_b200.h)."""
     _fields_ = [(n, C.c_int) for n in ('BN', 'TH', 'TW', 'TT', 'TB', 'tiles', 'kiters', 'stages', 'ks', 'ncbuf', 'nrbuf',
                                         'smem_bytes')] + [('useful_rows', C.c_double), ('stage_bytes', C.c_int)]
+
+
+class WgradPlan(C.Structure):
+    """dt_wgrad_plan_t (include/dt_b200.h)."""
+    _fields_ = [(n, C.c_int) for n in ('TW', 'TH', 'TT', 'TB', 'nW', 'nH', 'nT', 'nN', 'BN', 'taps', 'tiles_m', 'tiles_n', 'ksplit',
+                                        'grid', 'smem_bytes')]
 
 
 _RESTYPE = {'dt_last_error': C.c_char_p}

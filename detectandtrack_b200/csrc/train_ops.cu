@@ -291,12 +291,10 @@ wgrad_nhwc_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant
 }
 
 template <int BN>
-static int launch_wgrad_nhwc(const CUtensorMap& tmG, const CUtensorMap& tmX, const WgradNParams& p, cudaStream_t stream) {
-  constexpr int smem = WG_STAGES * (2 + BN / 64) * 64 * 128 + 256;
+static int launch_wgrad_nhwc(const CUtensorMap& tmG, const CUtensorMap& tmX, const WgradNParams& p, int smem, cudaStream_t stream) {
   static DynSmemGrant grant;
   DT_CHECK_CUDA(grant_dyn_smem(wgrad_nhwc_kernel<BN>, smem, &grant));
-  const long long grid = (long long)p.taps * p.tiles_m * p.tiles_n * p.ksplit;
-  DT_CHECK_ARG(grid < (1ll << 31), "dt_wgrad_nhwc: grid too large");
+  const long long grid = (long long)p.taps * p.tiles_m * p.tiles_n * p.ksplit;      // < 2^31: wgrad_nhwc_geom
   wgrad_nhwc_kernel<BN><<<(unsigned)grid, WG_THREADS, smem, stream>>>(tmG, tmX, p);
   DT_CHECK_LAUNCH();
   return 0;
@@ -855,6 +853,9 @@ __global__ void subpixel_grad_fix_kernel(float* __restrict__ gW, float* __restri
 
 using namespace dt;
 
+// the elementwise kernels move 16-byte vectors (uint4 / float4); NULL (an absent optional operand) passes
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
 static int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
   const long long cap = num_sms() * 16ll;
@@ -887,6 +888,7 @@ extern "C" int dt_wgrad(const void* gz_planes, const void* x_planes, int N, int 
                    (kT & 1) && (kH & 1) && (kW & 1),
                "dt_wgrad: bad shape N=%d T=%d %dx%d Cout=%d Cin=%d k=%dx%dx%d (odd 'same' kernels, Cin %% 8 == 0)", N, T, Ho, Wo, Cout, Cin, kT, kH, kW);
   DT_CHECK_ARG(gz_planes && x_planes && dW, "dt_wgrad: null pointer");
+  DT_CHECK_ARG(((uintptr_t)dW & 7) == 0, "dt_wgrad: dW must be 8-byte aligned (red.global.add.v2.f32)");
   const int pT = kT / 2, pH = kH / 2, pW = kW / 2;
   const int Pld = dt_planes_ld(Ho, Wo, pH, pW);
   const int Wp = (Wo + 2 * pW + 7) / 8 * 8, plane = Pld;
@@ -921,20 +923,20 @@ extern "C" int dt_wgrad(const void* gz_planes, const void* x_planes, int N, int 
   }
 }
 
-extern "C" int dt_wgrad_nhwc(const void* gz, int ld_g, const void* x, int ld_x, int N, int T, int Ho, int Wo, int Hi, int Wi, int Cout,
-                             int Cin, int kT, int kH, int kW, int sH, int sW, float* dW, void* stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
+// What dt_wgrad_nhwc launches, derived in one place for the launcher and dt_wgrad_nhwc_plan (the plan is what runs):
+// argument checks, the 64-position tile, BN, the tile counts, the K split, the grid and the dynamic shared memory.
+static int wgrad_nhwc_geom(int ld_g, int ld_x, int N, int T, int Ho, int Wo, int Hi, int Wi, int Cout, int Cin, int kT, int kH, int kW,
+                           int sH, int sW, WgradNParams* pp, int* BN_out, int* smem_out) {
   DT_CHECK_ARG(N >= 1 && T >= 1 && Ho >= 1 && Wo >= 1 && Cout >= 1 && Cin >= 8 && Cin % 4 == 0 && kT >= 1 && kH >= 1 && kW >= 1 && (kT & 1) &&
                    (kH & 1) && (kW & 1) && ld_g >= Cout && ld_g % 8 == 0 && ld_x >= Cin && ld_x % 8 == 0 && sH >= 1 && sW >= 1,
                "dt_wgrad_nhwc: bad shape N=%d T=%d %dx%d Cout=%d (ld %d) Cin=%d (ld %d) k=%dx%dx%d", N, T, Ho, Wo, Cout, ld_g, Cin, ld_x, kT, kH, kW);
   const bool strided = sH != 1 || sW != 1;
   DT_CHECK_ARG(!strided || (kT == 1 && kH == 1 && kW == 1), "dt_wgrad_nhwc: only pointwise convs may be strided");
   DT_CHECK_ARG(strided ? (Ho == (Hi + sH - 1) / sH && Wo == (Wi + sW - 1) / sW) : (Ho == Hi && Wo == Wi), "dt_wgrad_nhwc: output %dx%d does not match input %dx%d / stride", Ho, Wo, Hi, Wi);
-  DT_CHECK_ARG(gz && x && dW, "dt_wgrad_nhwc: null pointer");
-  WgradNParams p;
+  WgradNParams& p = *pp;
   memset(&p, 0, sizeof(p));
   p.Cout = Cout; p.Cin = Cin; p.taps = kT * kH * kW; p.kT = kT; p.kH = kH; p.kW = kW; p.pT = kT / 2; p.pH = kH / 2; p.pW = kW / 2;
-  p.T = T; p.dW = dW;
+  p.T = T;
   // 64-position tile (TW, TH, TT, TB), powers of two: the largest useful fraction, then the widest rows
   {
     double best = -1.0;
@@ -963,6 +965,35 @@ extern "C" int dt_wgrad_nhwc(const void* gz, int ld_g, const void* x, int ld_x, 
   if (ksplit > kblocks / 4) ksplit = kblocks / 4;
   if (ksplit < 1) ksplit = 1;
   p.ksplit = (int)ksplit;
+  DT_CHECK_ARG(units * ksplit < (1ll << 31), "dt_wgrad_nhwc: grid too large");
+  *BN_out = BN;
+  *smem_out = WG_STAGES * (2 + BN / 64) * 64 * 128 + 256;
+  return 0;
+}
+
+extern "C" int dt_wgrad_nhwc_plan(int ld_g, int ld_x, int N, int T, int Ho, int Wo, int Hi, int Wi, int Cout, int Cin, int kT, int kH,
+                                  int kW, int sH, int sW, dt_wgrad_plan_t* o) {
+  DT_CHECK_ARG(o, "dt_wgrad_nhwc_plan: null pointer");
+  WgradNParams p;
+  int BN = 0, smem = 0;
+  if (wgrad_nhwc_geom(ld_g, ld_x, N, T, Ho, Wo, Hi, Wi, Cout, Cin, kT, kH, kW, sH, sW, &p, &BN, &smem)) return 1;
+  o->TW = p.TW; o->TH = p.TH; o->TT = p.TT; o->TB = p.TB;
+  o->nW = p.nW; o->nH = p.nH; o->nT = p.nT; o->nN = p.nN;
+  o->BN = BN; o->taps = p.taps; o->tiles_m = p.tiles_m; o->tiles_n = p.tiles_n; o->ksplit = p.ksplit;
+  o->grid = p.taps * p.tiles_m * p.tiles_n * p.ksplit;
+  o->smem_bytes = smem;
+  return 0;
+}
+
+extern "C" int dt_wgrad_nhwc(const void* gz, int ld_g, const void* x, int ld_x, int N, int T, int Ho, int Wo, int Hi, int Wi, int Cout,
+                             int Cin, int kT, int kH, int kW, int sH, int sW, float* dW, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  WgradNParams p;
+  int BN = 0, smem = 0;
+  if (wgrad_nhwc_geom(ld_g, ld_x, N, T, Ho, Wo, Hi, Wi, Cout, Cin, kT, kH, kW, sH, sW, &p, &BN, &smem)) return 1;
+  DT_CHECK_ARG(gz && x && dW, "dt_wgrad_nhwc: null pointer");
+  DT_CHECK_ARG(((uintptr_t)dW & 7) == 0, "dt_wgrad_nhwc: dW must be 8-byte aligned (red.global.add.v2.f32)");
+  p.dW = dW;
   CUtensorMap tmG, tmX;
   const uint32_t box[5] = {64, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TT, (uint32_t)p.TB}, e[5] = {1, 1, 1, 1, 1};
   {
@@ -978,8 +1009,8 @@ extern "C" int dt_wgrad_nhwc(const void* gz, int ld_g, const void* x, int ld_x, 
     if (encode_map(&tmX, 0, 5, x, d, st, box, e)) return 1;
   }
   switch (BN) {
-    case 128: return launch_wgrad_nhwc<128>(tmG, tmX, p, stream);
-    default: return launch_wgrad_nhwc<64>(tmG, tmX, p, stream);
+    case 128: return launch_wgrad_nhwc<128>(tmG, tmX, p, smem, stream);
+    default: return launch_wgrad_nhwc<64>(tmG, tmX, p, smem, stream);
   }
 }
 
@@ -993,6 +1024,8 @@ extern "C" int dt_bwd_pointwise2(const void* g1, const void* g2, const void* y, 
   DT_CHECK_ARG(rows >= 0 && C >= 8 && C % 8 == 0, "dt_bwd_pointwise: bad shape rows=%lld C=%d (C %% 8 == 0)", rows, C);
   if (rows == 0) return 0;
   DT_CHECK_ARG(g1 && out, "dt_bwd_pointwise: null pointer");
+  DT_CHECK_ARG(aligned16(g1) && aligned16(g2) && aligned16(y) && aligned16(out) && aligned16(out2),
+               "dt_bwd_pointwise: g1 / g2 / y / out / out2 must be 16-byte aligned");
   bwd_pointwise_kernel<<<grid_for(rows * (C / 8), 256), 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)g1, (const __nv_bfloat16*)g2, (const __nv_bfloat16*)y, scale, rows, C, (__nv_bfloat16*)out, scale2,
       (__nv_bfloat16*)out2);
@@ -1004,6 +1037,7 @@ extern "C" int dt_upsample_add_bwd(const void* fine, const void* coarse_in, int 
   DT_CHECK_ARG(F >= 0 && Hc >= 1 && Wc >= 1 && C >= 8 && C % 8 == 0, "dt_upsample_add_bwd: bad shape");
   if (F == 0) return 0;
   DT_CHECK_ARG(fine && out, "dt_upsample_add_bwd: null pointer");
+  DT_CHECK_ARG(aligned16(fine) && aligned16(coarse_in) && aligned16(out), "dt_upsample_add_bwd: fine / coarse_in / out must be 16-byte aligned");
   upsample_add_bwd_kernel<<<grid_for((long long)F * Hc * Wc * (C / 8), 256), 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)fine, (const __nv_bfloat16*)coarse_in, F, Hc, Wc, C, (__nv_bfloat16*)out);
   DT_CHECK_LAUNCH();
@@ -1015,6 +1049,7 @@ extern "C" int dt_scatter_stride2(const void* src, int F, int Hs, int Ws, int H,
                "dt_scatter_stride2: bad shape %dx%d -> %dx%d C=%d", Hs, Ws, H, W, C);
   if (F == 0) return 0;
   DT_CHECK_ARG(src && out, "dt_scatter_stride2: null pointer");
+  DT_CHECK_ARG(aligned16(src) && aligned16(out), "dt_scatter_stride2: src / out must be 16-byte aligned");
   scatter_stride2_kernel<<<grid_for((long long)F * H * W * (C / 8), 256), 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)src, F, Hs, Ws, H, W, C, (__nv_bfloat16*)out);
   DT_CHECK_LAUNCH();
@@ -1025,6 +1060,7 @@ extern "C" int dt_embed_frame(const void* src, int B, int T, long long frame_ele
   DT_CHECK_ARG(B >= 0 && T >= 1 && c >= 0 && c < T && frame_elems >= 8 && frame_elems % 8 == 0, "dt_embed_frame: bad shape B=%d T=%d c=%d elems=%lld", B, T, c, frame_elems);
   if (B == 0) return 0;
   DT_CHECK_ARG(src && out, "dt_embed_frame: null pointer");
+  DT_CHECK_ARG(aligned16(src) && aligned16(out), "dt_embed_frame: src / out must be 16-byte aligned");
   embed_frame_kernel<<<grid_for((long long)B * T * (frame_elems / 8), 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)src, frame_elems / 8, B, T, c, (uint4*)out);
   DT_CHECK_LAUNCH();
   return 0;
@@ -1055,6 +1091,7 @@ extern "C" int dt_bias_grad(const void* g, long long rows, int C, int ld, float*
   DT_CHECK_ARG(rows >= 0 && C >= 8 && C % 8 == 0 && ld >= C && ld % 8 == 0, "dt_bias_grad: bad shape rows=%lld C=%d ld=%d (multiples of 8)", rows, C, ld);
   if (rows == 0) return 0;
   DT_CHECK_ARG(g && db, "dt_bias_grad: null pointer");
+  DT_CHECK_ARG(aligned16(g), "dt_bias_grad: g must be 16-byte aligned");
   long long gx = rows / 128; if (gx < 1) gx = 1; if (gx > num_sms() * 8ll) gx = num_sms() * 8ll;
   dim3 grid((unsigned)gx, (C + 255) / 256);
   bias_grad_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)g, rows, C, ld, db);
@@ -1078,6 +1115,7 @@ extern "C" int dt_grad_join_f32(const void* g, const float* acc, long long n, vo
   DT_CHECK_ARG(n >= 0 && n % 8 == 0, "dt_grad_join_f32: n=%lld must be a multiple of 8", n);
   if (n == 0) return 0;
   DT_CHECK_ARG(acc && out, "dt_grad_join_f32: null pointer");
+  DT_CHECK_ARG(aligned16(g) && aligned16(acc) && aligned16(out), "dt_grad_join_f32: g / acc / out must be 16-byte aligned");
   grad_join_f32_kernel<<<grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)g, acc, n / 8, (__nv_bfloat16*)out);
   DT_CHECK_LAUNCH();
   return 0;
@@ -1094,6 +1132,7 @@ extern "C" int dt_roi_align_bwd(const void* grad, float* const* dfeats, const in
   RoiBwdLevels lv;
   for (int l = 0; l < nlevels; ++l) {
     DT_CHECK_ARG(dfeats[l], "dt_roi_align_bwd: null accumulator for level %d", l);
+    DT_CHECK_ARG(aligned16(dfeats[l]), "dt_roi_align_bwd: accumulator of level %d must be 16-byte aligned (red.global.add.v4.f32)", l);
     lv.dfeat[l] = dfeats[l]; lv.H[l] = Hs[l]; lv.W[l] = Ws[l]; lv.scale[l] = scales[l];
   }
   dim3 grid(R * T, P);

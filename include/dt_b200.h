@@ -351,16 +351,28 @@ int dt_to_planes(const void* x, int F, int H, int W, int C, int ldx, int sh, int
  * sum_{n,t,h,w} gz[n,t,h,w,co] * x[n, t+kt-pT, h+kh-pH, w+kw-pW, ci].  gz_planes [N*T, Cout, Pld] (wshift 0), x_planes
  * [kW][N*T, Cin, Pld]: copy kw from dt_to_planes with pH = kH/2, pW = kW/2, wshift = kw - pW (strided 1x1 convs: x
  * subsampled by dt_to_planes).
- * dW is ACCUMULATED into (split-K partial sums, red.global): the caller zeroes it (dt_memset). */
+ * dW (8-byte aligned) is ACCUMULATED into (split-K partial sums, red.global): the caller zeroes it (dt_memset). */
 int dt_wgrad(const void* gz_planes, const void* x_planes, int N, int T, int Ho, int Wo, int Cout, int Cin, int kT, int kH, int kW,
              float* dW, void* stream);
 
 /* The same filter gradient read straight from the NDHWC tensors (no planes): gz [N, T, Ho, Wo, ld_g] (first Cout channels),
  * x [N, T, Hi, Wi, ld_x] (first Cin channels), both bf16.  Positions are the K axis of MN-major wgmma operands staged by
  * 5-D TMA boxes; the tap is a coordinate shift (zero fill = padding).  sH / sW > 1 only for pointwise convs
- * (Ho = ceil(Hi / sH)).  dW [taps][Cout][Cin] fp32 is accumulated into (caller zeroes). */
+ * (Ho = ceil(Hi / sH)).  dW [taps][Cout][Cin] fp32, 8-byte aligned, is accumulated into (caller zeroes). */
 int dt_wgrad_nhwc(const void* gz, int ld_g, const void* x, int ld_x, int N, int T, int Ho, int Wo, int Hi, int Wi, int Cout, int Cin,
                   int kT, int kH, int kW, int sH, int sW, float* dW, void* stream);
+
+/* Host-only planning query of dt_wgrad_nhwc (same shape arguments, no device work, usable without a GPU): the 64-position
+ * box TW x TH x TT frames x TB images, the box counts per axis (nW, nH, nT, nN; the K axis has nW*nH*nT*nN k-blocks),
+ * column tile BN, taps, output-channel / input-channel tiles, the K split (CTA ks of a (tap, tile) unit sums k-blocks
+ * [total*ks/ksplit, total*(ks+1)/ksplit)), the grid (taps * tiles_m * tiles_n * ksplit CTAs) and the dynamic shared memory. */
+typedef struct dt_wgrad_plan_t {
+  int TW, TH, TT, TB;
+  int nW, nH, nT, nN;
+  int BN, taps, tiles_m, tiles_n, ksplit, grid, smem_bytes;
+} dt_wgrad_plan_t;
+int dt_wgrad_nhwc_plan(int ld_g, int ld_x, int N, int T, int Ho, int Wo, int Hi, int Wi, int Cout, int Cin, int kT, int kH, int kW,
+                       int sH, int sW, dt_wgrad_plan_t* plan /*host out*/);
 
 /* out = (g1 + g2?) * [y > 0]? * scale[c]? over [rows, C] (any of g2 / y / scale may be NULL) */
 int dt_bwd_pointwise(const void* g1, const void* g2, const void* y, const float* scale, long long rows, int C, void* out,
@@ -414,7 +426,8 @@ int dt_grad_join_f32(const void* g, const float* acc, long long n, void* out, vo
 
 /* RoIAlign backward (the Caffe2 RoIAlignGradient the reference gets from AddGradientOperators for
  * lib/modeling/detector.py:216-310): grad [R, T, P, P, C] bf16 is scattered with the forward's bilinear weights into
- * fp32 accumulators dfeat[l] [Nimg*T, H_l, W_l, C] (caller zeroes them; red.global.add.v4.f32).  Arguments as dt_roi_align. */
+ * fp32 accumulators dfeat[l] [Nimg*T, H_l, W_l, C] (caller zeroes them, 16-byte aligned; red.global.add.v4.f32).  Arguments as
+ * dt_roi_align. */
 int dt_roi_align_bwd(const void* grad, float* const* dfeats /*host array [nlevels] of device ptrs*/, const int* Hs, const int* Ws,
                      const float* scales, int nlevels, int k_min, int C, const float* rois, int ldr, const int* n_dev, int R,
                      int T, const int* levels, int P, int sampling_ratio, void* stream);
