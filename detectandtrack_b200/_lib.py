@@ -68,9 +68,14 @@ SIGNATURES = {
     'dt_sample_rois': [_p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p, _i, _i, _i, _p, _i, _i, _f, _f, _f, _f, C.POINTER(_f), _i,
                        C.c_ulonglong, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p, _p],
 }
-# host-only helpers: no device work, usable without a GPU (dt_wgrad_nhwc_plan returns 0 or an error code like the rest)
+# host-only helpers: no device work, usable without a GPU (dt_wgrad_nhwc_plan returns 0 or an error code like the rest).
+# dt_prep_batch does launch a kernel; it is listed here rather than in SIGNATURES because its argument-error cases live
+# in tests/test_train_augment.py, one per host check, not in the single-case table of tests/test_capi_errors.py.
 HOST_FUNCS = {'dt_planes_ld': ([_i, _i, _i, _i], C.c_int), 'dt_jpeg_available': ([], C.c_int),
-              'dt_wgrad_nhwc_plan': ([_i] * 15 + [C.c_void_p], C.c_int)}
+              'dt_wgrad_nhwc_plan': ([_i] * 15 + [C.c_void_p], C.c_int),
+              'dt_prep_batch': ([C.POINTER(_p), C.POINTER(_i), C.POINTER(_i), C.POINTER(C.c_double), C.POINTER(_i), C.POINTER(_i),
+                                 C.POINTER(_i), _i, _i, C.POINTER(_f), _i, _i, _i, _i, _i, _i, _i, _p, _p], C.c_int)}
+PREP_MAX_CLIPS = 16                 # DT_PREP_MAX_CLIPS of include/dt_b200.h
 
 
 

@@ -2,6 +2,8 @@
 // accesses, one thread per 8 bf16 / 4 fp32 channels so every warp touches whole 128-byte lines):
 //   dt_prep_clip        lib/utils/blob.py:40-90 + lib/core/test.py:43-74: mean-subtract, cv2
 //                       INTER_LINEAR resize, zero pad to the /32 blob, BGR u8 -> NDHWC (C padded)
+//   dt_prep_batch       lib/roi_data/minibatch.py:66-90: the same per clip of a training minibatch, each clip
+//                       with its own source size, scale and horizontal flip, into one padded blob
 //   dt_maxpool2d        Caffe2 MaxPool [1,k,k] (lib/modeling/ResNet3D.py:264-265; FPN P6 subsample
 //                       lib/modeling/FPN3D.py:157-160)
 //   dt_roi_align        Caffe2 RoIAlign (Detectron module; lib/modeling/detector.py:216-310) incl.
@@ -80,67 +82,108 @@ __device__ __forceinline__ void store_vals(ET* p, int lo_off, float* v) {
 // frames [F, H, W, 3] u8 (BGR).  out [F, Hp, Wp, Cp]: channels 0..2 = resized (pixel - mean), rest 0;
 // rows/cols beyond the resized image are 0 (blob.py:40-62).  cv2.resize(INTER_LINEAR) on float32:
 // sx = (dx + 0.5) * (1/fx) - 0.5, floor, clamp, weights in float (see DESIGN.md, parity unpinned).
+//
+// One output pixel of frame f (both prep kernels call this, so their arithmetic is the same code).  The output
+// buffer is [F, Ht = Hp + 2*by, Wt = Wp + 2*bx, Cp]: `by` zero rows above/below, `bx` zero pixels left/right;
+// planes: the padded rows are de-interleaved, [F, 2 (row parity), Ht/2, Wt, Cp], so a stride-2 consumer
+// (conv1) reads contiguous rows of one parity plane per filter row.  flip: the SOURCE frame is mirrored before
+// the resize (minibatch.py:80-84, im[:, ::-1] then cv2.resize): the source column sx becomes W - 1 - sx with the
+// interpolation weights unchanged (cv2 maps output columns through 1/fx, not W/Wr, so this is not the mirror of
+// the resized image).
+template <typename OT>
+__device__ __forceinline__ void prep_pixel(const unsigned char* __restrict__ src, int H, int W, const float* mean,
+                                           double inv_scale, int Hr, int Wr, int flip, int f, int y, int x, int Ht,
+                                           int Wt, int by, int bx, int Cp, int round_out, int planes, int split_px,
+                                           size_t idx, OT* __restrict__ out) {
+  float v[3] = {0.f, 0.f, 0.f};
+  if (y >= 0 && x >= 0 && y < Hr && x < Wr) {
+    if (Hr == H && Wr == W) {
+      const unsigned char* p = src + ((size_t)y * W + (flip ? W - 1 - x : x)) * 3;
+      for (int c = 0; c < 3; ++c) v[c] = (float)p[c] - mean[c];
+    } else {
+      float fy = (float)((y + 0.5) * inv_scale - 0.5), fx = (float)((x + 0.5) * inv_scale - 0.5);
+      int sy = (int)floorf(fy), sx = (int)floorf(fx);
+      fy -= sy; fx -= sx;
+      if (sy < 0) { sy = 0; fy = 0.f; }
+      if (sy >= H - 1) { sy = H - 1 > 0 ? H - 2 : 0; fy = H > 1 ? 1.f : 0.f; if (H == 1) { sy = 0; } }
+      if (sx < 0) { sx = 0; fx = 0.f; }
+      if (sx >= W - 1) { sx = W - 1 > 0 ? W - 2 : 0; fx = W > 1 ? 1.f : 0.f; if (W == 1) { sx = 0; } }
+      const int sy1 = min(sy + 1, H - 1);
+      int sx1 = min(sx + 1, W - 1);
+      if (flip) { sx = W - 1 - sx; sx1 = W - 1 - sx1; }
+      for (int c = 0; c < 3; ++c) {
+        const float p00 = (float)src[((size_t)sy * W + sx) * 3 + c] - mean[c];
+        const float p01 = (float)src[((size_t)sy * W + sx1) * 3 + c] - mean[c];
+        const float p10 = (float)src[((size_t)sy1 * W + sx) * 3 + c] - mean[c];
+        const float p11 = (float)src[((size_t)sy1 * W + sx1) * 3 + c] - mean[c];
+        const float r0 = p00 * (1.f - fx) + p01 * fx;      // horizontal pass first (cv2 hresize)
+        const float r1 = p10 * (1.f - fx) + p11 * fx;
+        v[c] = r0 * (1.f - fy) + r1 * fy;                  // then vertical
+      }
+    }
+  }
+  size_t oidx = idx;
+  if (planes) {
+    const int yt = y + by;
+    oidx = (((size_t)f * 2 + (yt & 1)) * (Ht >> 1) + (yt >> 1)) * Wt + (x + bx);
+  }
+  OT* o = out + oidx * Cp;
+  if (round_out) { v[0] = round_to_tf32(v[0]); v[1] = round_to_tf32(v[1]); v[2] = round_to_tf32(v[2]); }
+  if (Cp * sizeof(OT) == 16) {                      // one 16-byte store per pixel
+    float q[Vec<OT>::N];
+#pragma unroll
+    for (int c = 0; c < Vec<OT>::N; ++c) q[c] = c < 3 ? v[c] : 0.f;
+    if constexpr (Vec<OT>::N >= 8) {
+      if (split_px) {                               // bf16x3 conv1 blob: [hi3 | lo3 | 0 0]
+#pragma unroll
+        for (int c = 0; c < 3; ++c) { const float h = split_hi<OT>(v[c]); q[c] = h; q[3 + c] = v[c] - h; }
+      }
+    }
+    Vec<OT>::store(o, q);
+  } else {
+    for (int c = 0; c < Cp; ++c) o[c] = to_act<OT>(c < 3 ? v[c] : 0.f);
+  }
+}
+
 template <typename OT>
 __global__ void prep_clip_kernel(const unsigned char* __restrict__ frames, int F, int H, int W, float m0, float m1,
                                  float m2, double inv_scale, int Hr, int Wr, int Hp, int Wp, int Cp,
                                  int by, int bx, int round_out, int planes, int split_px, OT* __restrict__ out) {
-  // the output buffer is [F, Hp + 2*by, Wp + 2*bx, Cp]: `by` zero rows above/below, `bx` zero pixels left/right;
-  // planes: the padded rows are de-interleaved, [F, 2 (row parity), Ht/2, Wt, Cp], so a stride-2 consumer
-  // (conv1) reads contiguous rows of one parity plane per filter row
   const int Ht = Hp + 2 * by, Wt = Wp + 2 * bx;
   const long long total = (long long)F * Ht * Wt;
+  const float mean[3] = {m0, m1, m2};
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
     const int x = (int)(idx % Wt) - bx;
     const int y = (int)((idx / Wt) % Ht) - by;
     const int f = (int)(idx / ((long long)Wt * Ht));
-    float v[3] = {0.f, 0.f, 0.f};
-    if (y >= 0 && x >= 0 && y < Hr && x < Wr) {
-      const unsigned char* src = frames + (size_t)f * H * W * 3;
-      const float mean[3] = {m0, m1, m2};
-      if (Hr == H && Wr == W) {
-        const unsigned char* p = src + ((size_t)y * W + x) * 3;
-        for (int c = 0; c < 3; ++c) v[c] = (float)p[c] - mean[c];
-      } else {
-        float fy = (float)((y + 0.5) * inv_scale - 0.5), fx = (float)((x + 0.5) * inv_scale - 0.5);
-        int sy = (int)floorf(fy), sx = (int)floorf(fx);
-        fy -= sy; fx -= sx;
-        if (sy < 0) { sy = 0; fy = 0.f; }
-        if (sy >= H - 1) { sy = H - 1 > 0 ? H - 2 : 0; fy = H > 1 ? 1.f : 0.f; if (H == 1) { sy = 0; } }
-        if (sx < 0) { sx = 0; fx = 0.f; }
-        if (sx >= W - 1) { sx = W - 1 > 0 ? W - 2 : 0; fx = W > 1 ? 1.f : 0.f; if (W == 1) { sx = 0; } }
-        const int sy1 = min(sy + 1, H - 1), sx1 = min(sx + 1, W - 1);
-        for (int c = 0; c < 3; ++c) {
-          const float p00 = (float)src[((size_t)sy * W + sx) * 3 + c] - mean[c];
-          const float p01 = (float)src[((size_t)sy * W + sx1) * 3 + c] - mean[c];
-          const float p10 = (float)src[((size_t)sy1 * W + sx) * 3 + c] - mean[c];
-          const float p11 = (float)src[((size_t)sy1 * W + sx1) * 3 + c] - mean[c];
-          const float r0 = p00 * (1.f - fx) + p01 * fx;      // horizontal pass first (cv2 hresize)
-          const float r1 = p10 * (1.f - fx) + p11 * fx;
-          v[c] = r0 * (1.f - fy) + r1 * fy;                  // then vertical
-        }
-      }
-    }
-    size_t oidx = (size_t)idx;
-    if (planes) {
-      const int yt = y + by;
-      oidx = (((size_t)f * 2 + (yt & 1)) * (Ht >> 1) + (yt >> 1)) * Wt + (x + bx);
-    }
-    OT* o = out + oidx * Cp;
-    if (round_out) { v[0] = round_to_tf32(v[0]); v[1] = round_to_tf32(v[1]); v[2] = round_to_tf32(v[2]); }
-    if (Cp * sizeof(OT) == 16) {                      // one 16-byte store per pixel
-      float q[Vec<OT>::N];
-#pragma unroll
-      for (int c = 0; c < Vec<OT>::N; ++c) q[c] = c < 3 ? v[c] : 0.f;
-      if constexpr (Vec<OT>::N >= 8) {
-        if (split_px) {                               // bf16x3 conv1 blob: [hi3 | lo3 | 0 0]
-#pragma unroll
-          for (int c = 0; c < 3; ++c) { const float h = split_hi<OT>(v[c]); q[c] = h; q[3 + c] = v[c] - h; }
-        }
-      }
-      Vec<OT>::store(o, q);
-    } else {
-      for (int c = 0; c < Cp; ++c) o[c] = to_act<OT>(c < 3 ? v[c] : 0.f);
-    }
+    prep_pixel<OT>(frames + (size_t)f * H * W * 3, H, W, mean, inv_scale, Hr, Wr, 0, f, y, x, Ht, Wt, by, bx, Cp, round_out,
+                   planes, split_px, (size_t)idx, out);
+  }
+}
+
+// dt_prep_batch: B clips of T frames, each with its own source size, scale, resized size and flip (a by-value table in
+// the kernel's parameter space: no H2D copy, no allocation), into one [B*T, Ht, Wt, Cp] blob of a shared padded size.
+struct PrepBatchClip {
+  const unsigned char* frames;
+  double inv_scale;
+  int H, W, Hr, Wr, flip;
+};
+struct PrepBatchTable { PrepBatchClip c[DT_PREP_MAX_CLIPS]; };
+
+template <typename OT>
+__global__ void prep_batch_kernel(const __grid_constant__ PrepBatchTable tab, int B, int T, float m0, float m1, float m2,
+                                  int Hp, int Wp, int Cp, int by, int bx, int round_out, int planes, int split_px,
+                                  OT* __restrict__ out) {
+  const int Ht = Hp + 2 * by, Wt = Wp + 2 * bx;
+  const long long total = (long long)B * T * Ht * Wt;
+  const float mean[3] = {m0, m1, m2};
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+    const int x = (int)(idx % Wt) - bx;
+    const int y = (int)((idx / Wt) % Ht) - by;
+    const int f = (int)(idx / ((long long)Wt * Ht));
+    const PrepBatchClip& c = tab.c[f / T];
+    prep_pixel<OT>(c.frames + (size_t)(f % T) * c.H * c.W * 3, c.H, c.W, mean, c.inv_scale, c.Hr, c.Wr, c.flip, f, y, x, Ht,
+                   Wt, by, bx, Cp, round_out, planes, split_px, (size_t)idx, out);
   }
 }
 
@@ -674,6 +717,42 @@ extern "C" int dt_prep_clip(const unsigned char* frames, int F, int H, int W, co
   else
     prep_clip_kernel<__nv_bfloat16><<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
         frames, F, H, W, mean3[0], mean3[1], mean3[2], 1.0 / im_scale, Hr, Wr, Hp, Wp, Cp, border_y, border_x, 0, row_planes, 0, (__nv_bfloat16*)out);
+  DT_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int dt_prep_batch(const unsigned char* const* frames, const int* H, const int* W, const double* im_scale,
+                             const int* Hr, const int* Wr, const int* flip, int B, int T, const float* mean3, int Hp, int Wp,
+                             int Cp, int border_y, int border_x, int row_planes, int out_f32, void* out, void* stream) {
+  DT_CHECK_ARG(B >= 1 && B <= DT_PREP_MAX_CLIPS && T >= 1, "dt_prep_batch: need 1 <= B <= %d clips and T >= 1 (B=%d T=%d)",
+               DT_PREP_MAX_CLIPS, B, T);
+  DT_CHECK_ARG(frames && H && W && im_scale && Hr && Wr && flip && mean3 && out, "dt_prep_batch: null pointer");
+  DT_CHECK_ARG(Hp >= 1 && Wp >= 1 && border_y >= 0 && border_x >= 0, "dt_prep_batch: bad padded size %dx%d or border %d,%d",
+               Hp, Wp, border_y, border_x);
+  PrepBatchTable tab;
+  for (int b = 0; b < B; ++b) {
+    DT_CHECK_ARG(frames[b], "dt_prep_batch: null frame pointer of clip %d", b);
+    DT_CHECK_ARG(H[b] >= 1 && W[b] >= 1, "dt_prep_batch: clip %d has source size %dx%d", b, H[b], W[b]);
+    DT_CHECK_ARG(im_scale[b] > 0, "dt_prep_batch: clip %d has im_scale %g <= 0", b, im_scale[b]);
+    DT_CHECK_ARG(Hr[b] >= 1 && Wr[b] >= 1 && Hr[b] <= Hp && Wr[b] <= Wp,
+                 "dt_prep_batch: clip %d resized size %dx%d does not fit the padded %dx%d", b, Hr[b], Wr[b], Hp, Wp);
+    tab.c[b] = PrepBatchClip{frames[b], 1.0 / im_scale[b], H[b], W[b], Hr[b], Wr[b], flip[b] ? 1 : 0};
+  }
+  DT_CHECK_ARG(!row_planes || (Hp + 2 * border_y) % 2 == 0, "dt_prep_batch: row planes need an even padded height");
+  DT_CHECK_ARG(Cp >= 3 && out_f32 >= 0 && out_f32 <= 3 && (out_f32 != 3 || Cp == 8),
+               "dt_prep_batch: bad output mode %d with Cp=%d (Cp >= 3; mode 3 needs Cp == 8)", out_f32, Cp);
+  const long long total = (long long)B * T * (Hp + 2 * border_y) * (Wp + 2 * border_x);
+  const int grid = grid_for(total, 256);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (out_f32 == 3)
+    prep_batch_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(tab, B, T, mean3[0], mean3[1], mean3[2], Hp, Wp, Cp, border_y, border_x, 0,
+                                                         row_planes, 1, (__nv_bfloat16*)out);
+  else if (out_f32)
+    prep_batch_kernel<float><<<grid, 256, 0, s>>>(tab, B, T, mean3[0], mean3[1], mean3[2], Hp, Wp, Cp, border_y, border_x,
+                                                 out_f32 == 1, row_planes, 0, (float*)out);
+  else
+    prep_batch_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(tab, B, T, mean3[0], mean3[1], mean3[2], Hp, Wp, Cp, border_y, border_x, 0,
+                                                         row_planes, 0, (__nv_bfloat16*)out);
   DT_CHECK_LAUNCH();
   return 0;
 }

@@ -16,6 +16,8 @@
 //     randint(n, k) = (hash(j) * n) >> 32 for j < k,
 // so the whole generator is deterministic and is compared bit for bit with the reference's own code run with exactly these
 // two draws (tests/golden/gen_golden_targets.py).  Compiled with -fmad=false.
+// Streams: 0 RPN fg disable, 1 RPN bg enable, 2 RoI fg, 3 RoI bg, 4 keypoint RoIs (these kernels); 5 the per-clip
+// TRAIN.SCALES draw of TRAIN.AUGMENT, made on the host (ops/target_ops.train_scale, image 0, index = clip counter).
 #include "common.cuh"
 #include "box_math.cuh"
 #include "../../include/dt_b200.h"

@@ -28,6 +28,24 @@ from . import params as P
 from .generate_anchors import generate_anchors
 
 
+def im_scale_and_size(h, w, target, max_size):
+    """prep_im_for_blob (blob.py:71-90) for one target size: (im_scale, (hr, wr)) of an h x w image."""
+    smin, smax = min(h, w), max(h, w)
+    scale = float(target) / float(smin)
+    if np.round(scale * smax) > max_size:
+        scale = float(max_size) / float(smax)
+    if scale == 1.0:
+        return scale, (h, w)
+    return scale, (int(round(h * scale)), int(round(w * scale)))     # cv2: saturate_cast<int>(size * fx)
+
+
+def padded_blob_size(sizes, stride):
+    """im_list_to_blob (blob.py:40-62): the (hp, wp) of a blob holding images of the resized `sizes` [(hr, wr)]: their
+    maximum, rounded up to a multiple of `stride` (FPN.COARSEST_STRIDE, or 1 without FPN)."""
+    hr, wr = max(s[0] for s in sizes), max(s[1] for s in sizes)
+    return int(np.ceil(hr / float(stride)) * stride), int(np.ceil(wr / float(stride)) * stride)
+
+
 class _Conv(object):
     """One packed convolution (+ fused epilogue parameters) resident on the device."""
 
@@ -428,18 +446,12 @@ class DetectionEngine(object):
     def blob_geometry(self, h, w):
         """prep_im_for_blob / im_list_to_blob geometry (blob.py:40-90): scale, resized, padded size."""
         cfg = self.cfg
-        target = cfg.TEST.SCALES[0]
-        smin, smax = min(h, w), max(h, w)
-        scale = float(target) / float(smin)
-        if np.round(scale * smax) > cfg.TEST.MAX_SIZE:
-            scale = float(cfg.TEST.MAX_SIZE) / float(smax)
-        if scale == 1.0:
-            hr, wr = h, w
-        else:
-            hr, wr = int(round(h * scale)), int(round(w * scale))     # cv2: saturate_cast<int>(size * fx)
-        stride = float(cfg.FPN.COARSEST_STRIDE) if cfg.FPN.FPN_ON else 1.0
-        hp, wp = int(np.ceil(hr / stride) * stride), int(np.ceil(wr / stride) * stride)
-        return scale, (hr, wr), (hp, wp)
+        scale, (hr, wr) = im_scale_and_size(h, w, cfg.TEST.SCALES[0], cfg.TEST.MAX_SIZE)
+        return scale, (hr, wr), padded_blob_size([(hr, wr)], self.blob_stride)
+
+    @property
+    def blob_stride(self):
+        return float(self.cfg.FPN.COARSEST_STRIDE) if self.cfg.FPN.FPN_ON else 1.0
 
     def plain(self, t):
         """Activation tensor as plain values (joins the [hi | lo] pairs of the 3xTF32 mode)."""
@@ -460,6 +472,19 @@ class DetectionEngine(object):
         mode = 3 if self.dtype == cv.BF16X3 else int(self.dtype == cv.TF32)
         x = dense_ops.prep_clip(frames_u8.view(B * T, H, W, 3), self.pixel_means, scale, (hr, wr), (hp, wp),
                                 cpad=self.cin_pad, out_f32=mode, border=(3, 4), row_planes=True)
+        return x.view(B, T, 2, (hp + 6) // 2, wp + 8, self.cin_pad)
+
+    def _blob_batch(self, clips, scales, sizes, flips, hp, wp):
+        """_blob for a training minibatch (minibatch.py:66-90): clips [T, H_b, W_b, 3] of their own sizes, each resized by
+        scales[b] to sizes[b] and mirrored where flips[b], into one blob of the padded size (hp, wp)."""
+        B, T = len(clips), clips[0].shape[0]
+        hp, wp = hp + (hp & 1), wp + (wp & 1)
+        if self.conv1_exact:
+            x = dense_ops.prep_batch(clips, self.pixel_means, scales, sizes, flips, (hp, wp), cpad=4, out_f32=2)
+            return x.view(B, T, hp, wp, 4)
+        mode = 3 if self.dtype == cv.BF16X3 else int(self.dtype == cv.TF32)
+        x = dense_ops.prep_batch(clips, self.pixel_means, scales, sizes, flips, (hp, wp), cpad=self.cin_pad, out_f32=mode,
+                                 border=(3, 4), row_planes=True)
         return x.view(B, T, 2, (hp + 6) // 2, wp + 8, self.cin_pad)
 
     def forward_features(self, frames_u8):

@@ -29,7 +29,7 @@ import numpy as np
 from .. import _lib as L
 from ..ops import conv as cv, dense_ops, train_ops as to, rpn_ops, box_ops, target_ops
 from . import params as P
-from .engine import DetectionEngine
+from .engine import DetectionEngine, im_scale_and_size, padded_blob_size
 from .generate_anchors import generate_anchors
 
 
@@ -225,13 +225,30 @@ class RpnTrainer(object):
     # ------------------------------------------------------------------ forward (activations saved for the backward)
     def forward_all(self, frames_u8):
         """stem -> res2 (frozen) -> res3..5 -> FPN -> RPN heads; returns per level the fp32 RPN outputs [B,1,H,W,ld]."""
-        torch, eng, s, cfg = self.torch, self.eng, self.spec, self.cfg
+        eng = self.eng
         B, T, H, W, _ = frames_u8.shape
-        self.rpn_conv.macs = self.rpn_out.macs = 0
         g = eng._geom_tensors(B, H, W)
         x = eng._blob(frames_u8, g['scale'], g['hr'], g['wr'], g['hp'], g['wp'])
+        return self.forward_blob(x, B, T, g['hp'], g['wp'])
+
+    def blob_clips(self, clips, targets, flipped):
+        """The training minibatch blob (minibatch.py:66-90): clip b ([T, H_b, W_b, 3] uint8 cuda) resized to its drawn
+        target size (TRAIN.MAX_SIZE bound), mirrored if flipped[b], all padded to one blob (im_list_to_blob).  Returns
+        (blob, hp, wp, im_info [B, 3] = (hr_b, wr_b, scale_b) per clip, the rows rpn.py:90 builds)."""
+        eng = self.eng
+        geo = [im_scale_and_size(c.shape[1], c.shape[2], t, self.cfg.TRAIN.MAX_SIZE) for c, t in zip(clips, targets)]
+        sizes = [hw for _, hw in geo]
+        hp, wp = padded_blob_size(sizes, eng.blob_stride)
+        x = eng._blob_batch(clips, [s for s, _ in geo], sizes, flipped, hp, wp)
+        im_info = self.torch.tensor([[hr, wr, s] for s, (hr, wr) in geo], dtype=self.torch.float32, device='cuda')
+        return x, hp, wp, im_info
+
+    def forward_blob(self, x, B, T, hp, wp):
+        """forward_all from a blob of _blob's layout with the padded size (hp, wp)."""
+        torch, eng, s, cfg = self.torch, self.eng, self.spec, self.cfg
+        self.rpn_conv.macs = self.rpn_out.macs = 0
         xs = x.view((B * T,) + tuple(x.shape[2:]))
-        y = cv.conv1_7x7s2(xs, eng.conv1_w, (g['hp'], g['wp']), eng.conv1_s, eng.conv1_b, relu=True, dtype=cv.BF16)
+        y = cv.conv1_7x7s2(xs, eng.conv1_w, (hp, wp), eng.conv1_s, eng.conv1_b, relu=True, dtype=cv.BF16)
         y = dense_ops.maxpool2d(y, 3, 2, 1)
         y = y.view((B, T) + tuple(y.shape[1:]))
         for blk in eng.stages[0]:
@@ -608,14 +625,17 @@ class KeypointRcnnTrainer(RpnTrainer):
 
     def make_targets(self, rpn_outs, gt, B, H, W, seed):
         """All targets of one step on the device: RPN anchor targets, sampled RoIs + box targets, keypoint RoIs + labels."""
+        return self.targets_at(rpn_outs, gt, self._train_geom(B, H, W)['im_info_train'], seed)
+
+    def targets_at(self, rpn_outs, gt, im_info, seed):
+        """make_targets with the per-clip im_info [B, 3] = (hr, wr, scale) rows (each target kernel reads its image's row)."""
         cfg, s = self.cfg, self.spec
-        g = self._train_geom(B, H, W)
         shapes = [(o.shape[2], o.shape[3]) for o in rpn_outs]
         rt = target_ops.rpn_targets(shapes, self.eng.anchors, [2. ** l for l in s.rpn_levels], self.A, gt['rpn_boxes'], gt['rpn_counts'],
-                                    g['im_info_train'], cfg.TRAIN, seed)
-        rois, scores, counts = self.proposals(rpn_outs, g['im_info_train'])
+                                    im_info, cfg.TRAIN, seed)
+        rois, scores, counts = self.proposals(rpn_outs, im_info)
         L.call('dt_memset', L.ptr(self.totals), 0, 8, L.stream_ptr())
-        smp = target_ops.sample_rois(rois, scores, counts, gt, g['im_info_train'], cfg, seed, keypoints=True, totals=self.totals)
+        smp = target_ops.sample_rois(rois, scores, counts, gt, im_info, cfg, seed, keypoints=True, totals=self.totals)
         return rt, smp
 
     # ------------------------------------------------------------------ heads
@@ -706,9 +726,20 @@ class KeypointRcnnTrainer(RpnTrainer):
     def step(self, frames_u8, gt, seed=None):
         """One SGD iteration from uint8 frames and packed ground truth (pack_gt): returns (rpn loss [2], head losses [4])."""
         B, T, H, W, _ = frames_u8.shape
-        seed = self.cfg.RNG_SEED + self.iter if seed is None else seed
         outs = self.forward_all(frames_u8)
-        rt, smp = self.make_targets(outs, gt, B, H, W, seed)
+        return self._step_from(outs, gt, self._train_geom(B, H, W)['im_info_train'], seed)
+
+    def step_clips(self, clips, gt, targets, flipped, seed=None):
+        """step() on a minibatch of clips of their own source sizes (TRAIN.AUGMENT): clip b ([T, H_b, W_b, 3] uint8 cuda)
+        is resized to targets[b] (its drawn TRAIN.SCALES entry) and mirrored if flipped[b]; gt (pack_gt) is already in
+        each clip's original, flipped-if-needed coordinates.  Returns what step() returns."""
+        x, hp, wp, im_info = self.blob_clips(clips, targets, flipped)
+        outs = self.forward_blob(x, len(clips), clips[0].shape[0], hp, wp)
+        return self._step_from(outs, gt, im_info, seed)
+
+    def _step_from(self, outs, gt, im_info, seed):
+        seed = self.cfg.RNG_SEED + self.iter if seed is None else seed
+        rt, smp = self.targets_at(outs, gt, im_info, seed)
         self.forward_heads(smp)
         L.call('dt_memset', L.ptr(self.flat_g), 0, self.flat_g.numel() * 4, L.stream_ptr())
         self.reducer.reset()

@@ -23,6 +23,27 @@ def prep_clip(frames_u8, pixel_means, im_scale, out_hw, pad_hw, cpad=8, out_f32=
     return out
 
 
+def prep_batch(clips, pixel_means, im_scales, out_hws, flips, pad_hw, cpad=8, out_f32=False, border=(0, 0), row_planes=False):
+    """clips: B uint8 cuda tensors [T, H_b, W_b, 3] (BGR; sizes may differ), each resized by im_scales[b] to out_hws[b],
+    its source mirrored horizontally first where flips[b] -> [B*T, ...] in prep_clip's layout at the shared pad_hw.
+    With flips[b] == 0, clip b's slice equals prep_clip of that clip byte for byte."""
+    torch = L.require_cuda()
+    B = len(clips)
+    T = clips[0].shape[0] if B else 0
+    assert all(c.dtype == torch.uint8 and c.dim() == 4 and c.shape[0] == T and c.shape[3] == 3 and c.is_contiguous() for c in clips)
+    Hp, Wp = pad_hw
+    by, bx = border
+    Ht, Wt = Hp + 2 * by, Wp + 2 * bx
+    shape = (B * T, 2, Ht // 2, Wt, cpad) if row_planes else (B * T, Ht, Wt, cpad)
+    out = torch.empty(shape, dtype=torch.float32 if out_f32 in (True, 1, 2) else torch.bfloat16, device='cuda')
+    ints = lambda v: (C.c_int * B)(*[int(x) for x in v])
+    L.call('dt_prep_batch', (C.c_void_p * B)(*[c.data_ptr() for c in clips]), ints([c.shape[1] for c in clips]),
+           ints([c.shape[2] for c in clips]), (C.c_double * B)(*[float(s) for s in im_scales]), ints([h for h, _ in out_hws]),
+           ints([w for _, w in out_hws]), ints([bool(f) for f in flips]), B, T, (C.c_float * 3)(*[float(v) for v in pixel_means]),
+           Hp, Wp, cpad, by, bx, int(bool(row_planes)), int(out_f32), L.ptr(out), L.stream_ptr())
+    return out
+
+
 def maxpool2d(x, k, s, p, x3=False):
     """x [N,H,W,C] -> [N,Ho,Wo,C] (floor mode).  x3: rows are [hi | lo] tf32 pairs (C = row / 2)."""
     torch = L.require_cuda()

@@ -5,6 +5,27 @@ import ctypes as C
 from .. import _lib as L
 from . import box_ops
 
+M64 = (1 << 64) - 1
+SCALE_STREAM = 5          # stream of the training-scale draw (streams 0..4 are csrc/targets.cu's)
+
+
+def hash_u32(seed, stream, image, i):
+    """csrc/targets.cu's counter-based generator on the host: splitmix64 finaliser over seed, stream, image and index
+    (unsigned 64-bit wrap-around) -> the high 32 bits."""
+    x = (seed * 0x9E3779B97F4A7C15 + stream * 0xBF58476D1CE4E5B9 + image * 0x94D049BB133111EB + i) & M64
+    x ^= x >> 30
+    x = (x * 0xBF58476D1CE4E5B9) & M64
+    x ^= x >> 27
+    x = (x * 0x94D049BB133111EB) & M64
+    x ^= x >> 31
+    return x >> 32
+
+
+def train_scale(scales, seed, n):
+    """The TRAIN.SCALES entry of the n-th clip of a run (n = it * world * B + rank * B + j): randint(len(SCALES)) on
+    stream 5, the reference's per-image npr.randint draw (minibatch.py:73-74) as a pure function of (seed, n)."""
+    return scales[(hash_u32(int(seed), SCALE_STREAM, 0, int(n)) * len(scales)) >> 32]
+
 
 def rpn_targets(level_shapes, anchors, strides, A, gt_boxes, gt_counts, im_info, cfg_train, seed, gt_visible=None):
     """level_shapes: [(H, W)] finest first; anchors: per level [A, 4T] fp64 device cell anchors; gt_boxes [B, Gmax, 4T] fp32

@@ -32,3 +32,14 @@ def boxes_area(boxes):
     areas = np.mean(w * h, axis=1)
     assert np.all(areas >= 0), 'Negative areas founds'
     return areas
+
+
+def flip_boxes(boxes, im_width):
+    """lib/utils/boxes.py:275-282 for boxes or T-frame tubes [n, 4T]: x1' = width - x2 - 1, x2' = width - x1 - 1 in every
+    frame's columns (0::4 and 2::4)."""
+    boxes = np.asarray(boxes)
+    flipped = boxes.copy()
+    flipped[:, 0::4] = im_width - boxes[:, 2::4] - 1
+    flipped[:, 2::4] = im_width - boxes[:, 0::4] - 1
+    assert np.all(flipped[:, 2::4] >= flipped[:, 0::4])
+    return flipped

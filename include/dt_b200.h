@@ -280,6 +280,17 @@ int dt_prep_clip(const unsigned char* frames, int F, int H, int W, const float* 
                  int Hr, int Wr, int Hp, int Wp, int Cp, int border_y, int border_x, int row_planes,
                  int out_f32, void* out, void* stream);
 
+/* The training minibatch blob (lib/roi_data/minibatch.py:66-90 _get_image_blob + blob.py im_list_to_blob): B clips of
+ * T frames, clip b = frames[b] [T, H[b], W[b], 3] u8 BGR (device pointer), resized by im_scale[b] to Hr[b] x Wr[b], its
+ * source frames mirrored horizontally first when flip[b] != 0, all zero padded to ONE Hp x Wp.  Host arrays of B
+ * entries, copied into the kernel's parameters (no H2D copy, no allocation); 1 <= B <= DT_PREP_MAX_CLIPS.
+ * Cp, border_y / border_x, row_planes and out_f32 as dt_prep_clip; out is [B*T, ...] in dt_prep_clip's layout, and
+ * with flip 0 clip b's slice equals dt_prep_clip of that clip byte for byte (the per-pixel code is shared). */
+#define DT_PREP_MAX_CLIPS 16
+int dt_prep_batch(const unsigned char* const* frames, const int* H, const int* W, const double* im_scale,
+                  const int* Hr, const int* Wr, const int* flip, int B, int T, const float* mean3, int Hp, int Wp,
+                  int Cp, int border_y, int border_x, int row_planes, int out_f32, void* out, void* stream);
+
 /* Caffe2 MaxPool kernels [1,k,k] strides [1,s,s] pads [0,p,p] on NHWC (N = B*T frames).
  * x3 != 0: split storage, rows are [hi(C) | lo(C)] pairs at ld/2 (tf32 pairs in fp32 tensors, bf16 pairs in bf16). */
 int dt_maxpool2d(const void* x, int N, int H, int W, int C, int ldx, int k, int s, int p, int f32, int x3,

@@ -8,6 +8,11 @@ The loop: minibatch (TRAIN.IMS_PER_BATCH clips + their ground truth) -> trainer.
 backward, bucketed gradient all-reduce, SGD with the lr of lib/utils/lr_policy) -> smoothed loss log every 20 iterations.
 TRAIN.DATASET 'synthetic_VxF[_HxW]' draws seeded frames and persons; any other name is a JSON list of roidb entries with
 'image', 'height', 'width', 'boxes', 'gt_keypoints' (the fields lib/datasets/json_dataset.py builds).
+
+TRAIN.AUGMENT True follows the reference's minibatch recipe (lib/datasets/roidb.py, lib/roi_data/minibatch.py): with
+TRAIN.USE_FLIPPED the roidb gets a horizontally flipped copy of every entry, each clip of a minibatch is resized to its own
+TRAIN.SCALES entry (drawn from (RNG_SEED, clip counter), so a resumed run repeats the draws), and clips of different
+source sizes share one blob.  False (the default) trains every clip unflipped at TRAIN.SCALES[-1].
 """
 import argparse
 import logging
@@ -59,6 +64,19 @@ def _synthetic_gt(entry, K):
     return dict(boxes=boxes, gt_keypoints=kps)
 
 
+def _entry_gt(entry, K, dataset_name):
+    """The ground truth of a TRAIN.AUGMENT minibatch entry: a JSON entry's own (already flipped in the roidb), or the seeded
+    synthetic gt, flipped like the entry's roidb copy when the entry is a flipped one."""
+    if not entry.get('synthetic'):
+        return dict(boxes=np.asarray(entry['boxes'], np.float32), gt_keypoints=np.asarray(entry['gt_keypoints'], np.int32))
+    gt = _synthetic_gt(entry, K)
+    if entry.get('flipped'):
+        from detectandtrack_b200.utils.roidb import flipped_entry, keypoint_flip_pairs
+        f = flipped_entry(dict(gt, width=entry['width']), keypoint_flip_pairs(dataset_name), K)
+        gt = dict(boxes=f['boxes'], gt_keypoints=f['gt_keypoints'])
+    return gt
+
+
 def train_model():
     import torch
     import torch.distributed as dist
@@ -71,7 +89,8 @@ def train_model():
     torch.cuda.set_device(int(os.environ.get('LOCAL_RANK', '0')))
     if world > 1:
         dist.init_process_group('nccl')
-    cfg.TEST.SCALES, cfg.TEST.MAX_SIZE = (cfg.TRAIN.SCALES[-1],), cfg.TRAIN.MAX_SIZE       # one training scale per run (the blob geometry)
+    # the blob geometry of TRAIN.AUGMENT False: one training scale per run (AUGMENT draws one per clip, trainer.blob_clips)
+    cfg.TEST.SCALES, cfg.TEST.MAX_SIZE = (cfg.TRAIN.SCALES[-1],), cfg.TRAIN.MAX_SIZE
     from detectandtrack_b200.core.config import get_output_dir
     from detectandtrack_b200.modeling import params as P
     import yaml
@@ -90,7 +109,13 @@ def train_model():
         path = os.path.join(output_dir, name)
         P.save_weights_file(model.export_blobs(model.blobs0), yaml.dump({'MODEL': {'TYPE': cfg.MODEL.TYPE, 'CONV_BODY': cfg.MODEL.CONV_BODY}}), path)
         log.info('Wrote %s', path)
-    roidb = te.get_dataset(cfg.TRAIN.DATASET).get_roidb(gt=True)
+    augment = bool(cfg.TRAIN.AUGMENT)
+    dataset = te.get_dataset(cfg.TRAIN.DATASET)
+    if augment:
+        from detectandtrack_b200.utils.roidb import training_roidb
+        roidb = training_roidb(dataset, bool(cfg.TRAIN.USE_FLIPPED))
+    else:
+        roidb = dataset.get_roidb(gt=True)
     K = cfg.KRCNN.NUM_KEYPOINTS
     B = cfg.TRAIN.IMS_PER_BATCH
     order = np.random.RandomState(cfg.RNG_SEED).permutation(len(roidb))
@@ -98,11 +123,18 @@ def train_model():
     for it in range(start_iter, cfg.SOLVER.MAX_ITER):
         idx = [order[(it * world * B + rank * B + j) % len(order)] for j in range(B)]
         entries = [roidb[i] for i in idx]
-        frames = torch.from_numpy(np.stack([np.stack(te.read_image_video(e)) for e in entries])).cuda()
-        gts = [(_synthetic_gt(e, K) if e.get('synthetic') else dict(boxes=np.asarray(e['boxes'], np.float32),
-                                                                    gt_keypoints=np.asarray(e['gt_keypoints'], np.int32))) for e in entries]
         model.lr = float(get_lr_at_iter(it))
-        l_rpn, l_heads = model.step(frames, pack_gt(gts, K=K))
+        if augment:           # minibatch.py:66-90: per clip its own frames, drawn scale and flip; the gt is flipped on the host
+            from detectandtrack_b200.ops.target_ops import train_scale
+            clips = [torch.from_numpy(np.ascontiguousarray(np.stack(te.read_image_video(e)))).cuda() for e in entries]
+            targets = [train_scale(cfg.TRAIN.SCALES, cfg.RNG_SEED, it * world * B + rank * B + j) for j in range(B)]
+            gts = [_entry_gt(e, K, dataset.name) for e in entries]
+            l_rpn, l_heads = model.step_clips(clips, pack_gt(gts, K=K), targets, [bool(e.get('flipped')) for e in entries])
+        else:
+            frames = torch.from_numpy(np.stack([np.stack(te.read_image_video(e)) for e in entries])).cuda()
+            gts = [(_synthetic_gt(e, K) if e.get('synthetic') else dict(boxes=np.asarray(e['boxes'], np.float32),
+                                                                        gt_keypoints=np.asarray(e['gt_keypoints'], np.int32))) for e in entries]
+            l_rpn, l_heads = model.step(frames, pack_gt(gts, K=K))
         if rank == 0 and (it + 1) % snap_every == 0 and it > start_iter:      # :208-212
             snapshot('model_iter{}.pkl'.format(it))
         if it % 20 == 0 or it == cfg.SOLVER.MAX_ITER - 1:
