@@ -110,7 +110,8 @@ class ConvDesc(C.Structure):
 class ConvPlan(C.Structure):
     """dt_conv_plan_t (include/dt_b200.h)."""
     _fields_ = [(n, C.c_int) for n in ('BN', 'TH', 'TW', 'TT', 'TB', 'tiles', 'kiters', 'stages', 'ks', 'ncbuf', 'nrbuf',
-                                        'smem_bytes')] + [('useful_rows', C.c_double), ('stage_bytes', C.c_int)]
+                                        'smem_bytes')] + [('useful_rows', C.c_double), ('stage_bytes', C.c_int),
+                                                          ('mma_kblocks', C.c_double)]
 
 
 class WgradPlan(C.Structure):

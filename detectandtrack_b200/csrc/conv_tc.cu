@@ -89,7 +89,22 @@ struct ConvKernelParams {
   int ab_format;               // 16-bit operand format: 1 bf16, 0 fp16 (TF32 kernels ignore it)
   int round_tf32;              // fp32 output is rounded (RNE) to tf32 so the next tf32 MMA, which ignores the
                                // low mantissa bits of its 32-bit operands, sees exactly representable values
+  int Ti, Hi, Wi;              // input size: a tap whose activation box lies wholly outside it is skipped (tile_live)
+  int all_live;                // every tap of every tile is issued: conv1 (row-plane table) and pointwise convs
+                               // (maps in output coordinates, no padding)
 };
+
+// Taps [k0, k0 + n) of one filter dimension that are live for a tile.  The activation box of tap k covers the input
+// coordinates base + k .. base + k + (ext - 1) * s (base = tile origin * stride - pad); when all of them lie below 0
+// or at / beyond the input size the TMA unit zero-fills the whole box and the tap's MMAs would only add zeros.  The
+// whole box counts, the rows of a ragged edge tile outside the output included, so a tap is never skipped wrongly.
+struct TapRange { int k0, n; };
+__host__ __device__ __forceinline__ TapRange live_taps(int base, int ext, int s, int size, int k) {
+  const int last = base + (ext - 1) * s;
+  const int k0 = last < 0 ? -last : 0;              // first tap whose box reaches coordinate 0
+  const int k1 = size - base < k ? size - base : k; // taps from here on start at / beyond the input size
+  return {k0, k1 > k0 ? k1 - k0 : 0};
+}
 
 __device__ __forceinline__ float round_to_tf32(float v) {
   uint32_t u = __float_as_uint(v);
@@ -162,6 +177,16 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvKernelParams& p, int 
   q = fdiv(m, p.fd_t);                        c.tti = (int)m - (int)q * p.tiles_t;
   c.tbi = (int)q;
   return c;
+}
+
+// The live taps of a tile: the product of one TapRange per dimension.  The T box spans TT frames at unit element
+// stride; frames are stacked (TT > 1) only with sT = 1, so (TT - 1) * sT is its extent either way.
+struct LiveTaps { TapRange t, h, w; };
+__device__ __forceinline__ LiveTaps tile_live(const ConvKernelParams& p, const TileCoord& tc) {
+  if (p.all_live) return {{0, p.kT}, {0, p.kH}, {0, p.kW}};
+  return {live_taps((tc.tti * p.TT + p.t_first) * p.sT - p.pT, p.TT, p.sT, p.Ti, p.kT),
+          live_taps(tc.thi * p.TH * p.sH - p.pH, p.TH, p.sH, p.Hi, p.kH),
+          live_taps(tc.twi * p.TW * p.sW - p.pW, p.TW, p.sW, p.Wi, p.kW)};
 }
 
 // SPLIT: the output (and the residual) rows are [hi | lo] pairs (the x3 modes' intermediate activations); a template
@@ -243,8 +268,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  const int groups = p.kT * p.kH * p.kW * p.kchunks;    // (tap, channel chunk) groups per tile
-
   if (warp == 0 || warp == B_WARP) {
     // ===================== TMA producers =====================
     // Two warps: warp 0 loads the activation tiles (and the residual ring), warp B_WARP the weight tiles; both
@@ -269,17 +292,36 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int h_base = tc.thi * p.TH * p.sH - p.pH;
       const int t_base = p.row_planes ? 0 : (tc.tti * p.TT + p.t_first) * p.sT - p.pT;
       const int n_base = tc.nt * BN;
-      for (int ki = 0; ki < groups; ki += KS) {
-        const int nk = min(KS, groups - ki);
+      // the live groups of the tile: for each live (kt, kh), a run of lv.w.n * kchunks consecutive schedule entries
+      // (kw, then the channel chunk innermost).  j walks them; at the end of a run it jumps over the dead kw taps to the
+      // next live kh row, and after the last live row of a kt plane over the dead kh rows as well.
+      const LiveTaps lv = tile_live(p, tc);
+      const int run = lv.w.n * p.kchunks;
+      const int live = lv.t.n * lv.h.n * run;
+      const int skip_h = (p.kW - lv.w.n) * p.kchunks;
+      const int skip_t = skip_h + (p.kH - lv.h.n) * p.kW * p.kchunks;
+      int j = ((lv.t.k0 * p.kH + lv.h.k0) * p.kW + lv.w.k0) * p.kchunks;
+      int run_end = j + run, rows = lv.h.n;
+      for (int ki = 0; ki < live; ki += KS) {
+        const int nk = min(KS, live - ki);
         // this stage's groups from the schedule (uniform loads), then ONE elected issue block
+        int jq[2];
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          jq[q] = q < nk ? j : jq[0];                  // an unused second slot re-reads the first entry (never issued)
+          if (q < nk && ++j == run_end) {
+            if (--rows == 0) { rows = lv.h.n; j += skip_t; } else { j += skip_h; }
+            run_end = j + run;
+          }
+        }
         int x0[2], x1[2], x2[2], x3[2];
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
           if (load_b) {
-            const int2 e = tabB[ki + q];
+            const int2 e = tabB[jq[q]];
             x0[q] = e.x; x1[q] = n_base; x2[q] = e.y; x3[q] = 0;
           } else {
-            const int4 e = tabA[ki + q];
+            const int4 e = tabA[jq[q]];
             x0[q] = e.x; x1[q] = w_base + e.y; x2[q] = h_base + e.z; x3[q] = t_base + e.w;
           }
         }
@@ -412,8 +454,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       // ---- main loop: one wgmma group per (tap, channel chunk) group; a ring stage goes back to the producers once
       // the wgmma group of the NEXT stage's last group is issued and the stage's own wgmma groups retired (one stage
       // stays in flight).  The wgmmas sit outside any branch so that they are not serialized.
+      // only the tile's live groups are issued (the producers walk the same ones, tile_live); ki, and with it the
+      // pairing into ring stages and scale-d of the first wgmma, counts from the first live group
+      const LiveTaps lv = tile_live(p, tc);
+      const int live = lv.t.n * lv.h.n * lv.w.n * p.kchunks;
+      if (live == 0) {
+        // no live group (every box of the tile lies in the zero padding, e.g. a 1x1x1 conv with temporal padding on its
+        // first / last frame): the conv is 0 and no ring stage is used.  The epilogue still runs on that (scale * 0 +
+        // bias, residual, ReLU), not on the previous tile's accumulators
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      }
       int prev = -1;
-      for (int ki = 0; ki < groups; ++ki) {
+      for (int ki = 0; ki < live; ++ki) {
         const int q = KS == 2 ? (ki & 1) : 0;          // group inside the ring stage
         if (q == 0) mbar_wait_u(full_u + stage * 8, phase);
         const uint32_t off = stage * stage_bytes + q * group_bytes;
@@ -430,7 +483,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             wgmma<BN, KIND>(acc, adesc + 2 * k, bdesc + 2 * k, (ki | s | k) != 0 ? 1u : 0u);
         }
         wgmma_commit();
-        if (q == KS - 1 || ki == groups - 1) {
+        if (q == KS - 1 || ki == live - 1) {
           if (q == 1) wgmma_wait<2>(); else wgmma_wait<1>();   // only this stage's q + 1 groups may still run
           if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
           prev = stage;
@@ -439,7 +492,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[prev]);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
 
       // ---- epilogue
       bool valid[2] = {true, true};
@@ -612,6 +665,7 @@ struct ConvGeom {
   int kchunks, groups, nmma;   // (tap, channel chunk) groups per tile, MMA k-blocks per group
   bool res_tma;                // bf16 residual chunks arrive through the TMA ring
   bool res_up;                 // ... as the (TH/2 x TW/2) box of the coarser map of the FPN top-down add
+  bool all_live;               // no tap is ever skipped (pointwise: the map is in output coordinates, without padding)
 };
 static ConvGeom conv_geom(const dt_conv_desc* d, bool residual_aligned) {
   ConvGeom g;
@@ -640,7 +694,24 @@ static ConvGeom conv_geom(const dt_conv_desc* d, bool residual_aligned) {
   const bool res_even = (g.ts.th % 2 == 0) && (g.ts.tw % 2 == 0);
   g.res_tma = (d->res_mode == 1 || (d->res_mode == 2 && res_even)) && !d->out_f32 && !g.tf32 && residual_aligned;
   g.res_up = g.res_tma && d->res_mode == 2;
+  g.all_live = g.pointwise;
   return g;
+}
+
+// MMA k-blocks one launch issues: nmma per live (tap, channel chunk) group of every tile.  The live taps of a tile are a
+// product of one range per dimension (live_taps, as the kernel's tile_live), so the sum over tiles is a product of
+// per-dimension sums.
+static double conv_mma_kblocks(const dt_conv_desc* d, const ConvGeom& g) {
+  const TileShape& ts = g.ts;
+  const int t_first = d->out_t_count > 0 ? d->out_t_first : 0;
+  double st = 0, sh = 0, sw = 0;
+  for (int i = 0; i < cdiv(g.To, ts.tt); ++i)
+    st += g.all_live ? d->kT : live_taps((i * ts.tt + t_first) * d->sT - d->pT, ts.tt, d->sT, d->Ti, d->kT).n;
+  for (int i = 0; i < cdiv(g.Ho, ts.th); ++i)
+    sh += g.all_live ? d->kH : live_taps(i * ts.th * d->sH - d->pH, ts.th, d->sH, d->Hi, d->kH).n;
+  for (int i = 0; i < cdiv(g.Wo, ts.tw); ++i)
+    sw += g.all_live ? d->kW : live_taps(i * ts.tw * d->sW - d->pW, ts.tw, d->sW, d->Wi, d->kW).n;
+  return (double)g.nmma * g.kchunks * cdiv(d->Cout, g.BN) * cdiv(d->N, ts.tb) * st * sh * sw;
 }
 
 template <int BN, int KIND, bool SPLIT, int NMMA>
@@ -765,6 +836,8 @@ extern "C" int dt_conv3d(const dt_conv_desc* d, const void* x, const void* w, co
   const int BN = g.BN;
   const bool res_tma = g.res_tma;
   p.t_first = d->out_t_count > 0 ? d->out_t_first : 0;
+  p.Ti = d->Ti; p.Hi = d->Hi; p.Wi = d->Wi;
+  p.all_live = g.all_live ? 1 : 0;
   p.nrbuf = res_tma ? 1 : 0;                         // ring depth is chosen with the smem split at launch
   p.res_up = g.res_up ? 1 : 0;
   p.tiles_n = cdiv(d->Cout, BN);
@@ -858,6 +931,7 @@ extern "C" int dt_conv_plan(const dt_conv_desc* d, int residual_aligned, dt_conv
     case 64: plan_split<64>(g.groups, g.nmma, g.res_tma, g.split_out, d->out_f32 != 0, o); break;
     default: plan_split<32>(g.groups, g.nmma, g.res_tma, g.split_out, d->out_f32 != 0, o); break;
   }
+  o->mma_kblocks = conv_mma_kblocks(d, g);
   return 0;
 }
 
@@ -900,6 +974,8 @@ extern "C" int dt_conv1_7x7s2(const void* x_padded, int F, int Hp, int Wp, int C
   p.N = F; p.To = 1; p.Ho = Ho; p.Wo = Wo; p.Cout = Cout;
   p.kT = 1; p.kH = 7; p.kW = 1; p.sT = 1; p.sH = 1; p.sW = 1; p.pT = 0; p.pH = 0; p.pW = 0;
   p.row_planes = 1;
+  p.all_live = 1;                                  // the schedule's h / t slots are row-plane offsets, the blob carries
+                                                   // its zero border: every filter row is issued
   p.kchunks = 1;
   p.ab_format = 1;
   p.b_lo_blk = 1;                                  // x3: weight blocks 2*kh and 2*kh + 1 against one activation box

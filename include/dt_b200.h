@@ -183,6 +183,8 @@ int dt_conv3d(const dt_conv_desc* desc /*host*/, const void* x, const void* w, c
  * (stages x ks (tap, channel chunk) groups of stage_bytes / ks bytes: one activation and one weight box, or with x3
  * inputs the hi and lo box of each), output staging / residual ring chunks, dynamic shared memory, MMA k-blocks per
  * tile (three per group with x3 inputs) and the fraction of MMA rows that are real output positions.
+ * kiters is the per-tile maximum; a tap whose activation box lies wholly in the zero padding (or past the input) is
+ * not issued, and mma_kblocks counts the MMA k-blocks the whole launch does issue.
  * residual_aligned: the residual pointer would be 16-byte aligned (enables the TMA residual ring for bf16 residual
  * modes). */
 typedef struct dt_conv_plan_t {
@@ -190,6 +192,7 @@ typedef struct dt_conv_plan_t {
   int tiles, kiters, stages, ks, ncbuf, nrbuf, smem_bytes;
   double useful_rows;
   int stage_bytes;
+  double mma_kblocks;
 } dt_conv_plan_t;
 int dt_conv_plan(const dt_conv_desc* desc /*host*/, int residual_aligned, dt_conv_plan_t* plan /*host out*/);
 
