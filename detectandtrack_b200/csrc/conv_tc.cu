@@ -21,9 +21,11 @@
 //   warp 0, 1 : TMA producers (activation / weight tiles; one elected lane each)   smem ring: full[]/empty[]
 //   warp 2    : TMA store warp                           staged output chunks -> global, recycles staging slots
 //   warp 3    : idle (pads the producer warpgroup)
-//   warps 4-11: two consumer warpgroups, rows 0-63 and 64-127 of the tile: wgmma into register accumulators
-//               (64 x BLOCK_N each), then the epilogue: scale/bias/residual/ReLU in fp32, staged in 128B-swizzled
-//               smem chunks.  The producers run ahead into the next tile's k-blocks while the epilogue runs.
+//   warps 4-11: two consumer warpgroups in ping-pong: each takes every other tile of the CTA's sequence and runs the
+//               whole 128-row tile, wgmma into register accumulators (two 64 x BLOCK_N halves), then the epilogue:
+//               scale/bias/residual/ReLU in fp32, staged in 128B-swizzled smem chunks.  One warpgroup's epilogue runs
+//               while the other issues the next tile's MMAs.  The producer warpgroup gives registers to the consumers
+//               (setmaxnreg).
 // Everything is handed over through mbarriers; there is no block-wide barrier inside the tile loop.
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -116,6 +118,13 @@ constexpr int EPI_WARPS = 8;                          // two consumer warpgroups
 constexpr int CONV_THREADS = 128 + EPI_WARPS * 32;    // + the producer warpgroup (two TMA producer warps, the TMA store warp)
 constexpr int B_WARP = 1;                             // weight-tile producer
 constexpr int EPI_WARP0 = 4;                          // first consumer warp
+constexpr int WG_WARPS = 4;                           // warps of one consumer warpgroup: the arrivals a tile's barriers expect
+// registers per thread after setmaxnreg: the producer warpgroup only walks schedules and issues TMA; a consumer holds a
+// whole tile's 128 x BN fp32 accumulators (BN per thread).  The split must fit the CTA's pool at launch, 384 threads x
+// 168 (the __launch_bounds__ cap); both counts are multiples of 8.  The producer loops spill at 40.
+constexpr int PRODUCER_REGS = 56;
+constexpr int CONSUMER_REGS = 224;
+static_assert(128 * PRODUCER_REGS + EPI_WARPS * 32 * CONSUMER_REGS <= CONV_THREADS * 168, "register split exceeds the pool");
 
 template <int BN>
 struct ConvCfg {
@@ -194,7 +203,12 @@ __device__ __forceinline__ LiveTaps tile_live(const ConvKernelParams& p, const T
 // KIND: MMA operand type, 0 bf16, 1 fp16, 2 tf32 (wgmma.cuh).
 // NMMA: MMA k-blocks per (tap, channel chunk) group, 1 plain, 3 split operands, 2 split conv1 (ConvCfg::group_bytes);
 // a template parameter so that the products of a group are straight-line wgmmas.
-template <int BN, int KIND, bool SPLIT, int NMMA>
+// OUT_F32 (p.out_f32) and RES (0 no residual, RES_TMA the TMA residual ring, RES_LDG per-thread residual loads): the
+// epilogue's path.  The epilogue is unrolled over a whole tile's 64 (row, 8-column group) pairs per thread, so every
+// runtime branch in it is 64 copies of code; compiled for one path it is a third of the size, and one warpgroup running
+// it alone measured 2.5x slower on the K-light layers when it carried all paths.
+constexpr int RES_TMA = 1, RES_LDG = 2;
+template <int BN, int KIND, bool SPLIT, int NMMA, bool OUT_F32, int RES>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
@@ -219,6 +233,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* r_empty = r_full + 4;              // [4]       residual chunk consumed
   uint64_t* c_full = r_full + 8;               // [4]       output chunk staged by all epilogue warps
   uint64_t* c_free = r_full + 12;              // [4]       staging slot read out by its TMA store
+  uint64_t* ml_ord = r_full + 16;              // [2]       consumer warpgroup g's mainloop has waited on all its ring stages
+  uint64_t* ep_ord = r_full + 18;              // [2]       consumer warpgroup g's epilogue has staged all its chunks
   // schedule of one tile, one entry per (tap, channel chunk) group: what the producers add to the tile's base
   // coordinates for the group's first boxes (its lo boxes sit at the lo offsets from there).
   // Built once; walking taps / channel chunks with carry logic in the producer loop costs more cycles per
@@ -253,11 +269,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     prefetch_tmap(&tmB);
     prefetch_tmap(&tmC);
     if (p.nrbuf > 0) prefetch_tmap(&tmR);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 2); mbar_init(&empty[s], EPI_WARPS); }  // full: A and B producers
+    // a tile's stages, residual chunks and staging slots are released by the warps of the one warpgroup that runs it
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 2); mbar_init(&empty[s], WG_WARPS); }  // full: A and B producers
     for (int s = 0; s < 4; ++s) {
-      mbar_init(&r_full[s], 1); mbar_init(&r_empty[s], EPI_WARPS);
-      mbar_init(&c_full[s], EPI_WARPS); mbar_init(&c_free[s], 1);
+      mbar_init(&r_full[s], 1); mbar_init(&r_empty[s], WG_WARPS);
+      mbar_init(&c_full[s], WG_WARPS); mbar_init(&c_free[s], 1);
     }
+    for (int g = 0; g < 2; ++g) { mbar_init(&ml_ord[g], WG_WARPS); mbar_init(&ep_ord[g], WG_WARPS); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -268,202 +286,236 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  if (warp == 0 || warp == B_WARP) {
-    // ===================== TMA producers =====================
-    // Two warps: warp 0 loads the activation tiles (and the residual ring), warp B_WARP the weight tiles; both
-    // arm the same full[] barrier with their own byte count, so the scalar bookkeeping of the two operands runs
-    // in parallel.  The whole warp runs the loop (warp-uniform control flow and addresses, so descriptors /
-    // coordinates stay in uniform registers); one elected lane issues.
-    const bool load_b = warp != 0;
-    int stage = 0; uint32_t phase = 0;
-    int rslot = 0; uint32_t rphase = 0;
-    const uint32_t smem_u = smem_u32(smem) + (load_b ? (uint32_t)(NA * Cfg::A_BYTES) : 0u);
-    const uint32_t full_u = smem_u32(full), empty_u = smem_u32(empty);
-    const int KS = p.ks;                                  // groups per ring stage (one mbarrier round trip)
-    const int nbox = load_b ? NB : NA;                    // this warp's boxes per group: hi, then lo
-    const uint32_t box_bytes = load_b ? (uint32_t)Cfg::B_BYTES : (uint32_t)Cfg::A_BYTES;
-    const uint32_t box_tx = load_b ? (uint32_t)Cfg::B_BYTES : p.a_bytes;
-    const int lo_c = load_b ? p.b_lo_off : p.a_lo_off;    // the lo box: channel offset / weight block offset
-    const int lo_blk = load_b ? p.b_lo_blk : 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const TileCoord tc = decode_tile(p, tile);
-      const int n = tc.tbi * p.TB;
-      const int w_base = tc.twi * p.TW * p.sW - p.pW;
-      const int h_base = tc.thi * p.TH * p.sH - p.pH;
-      const int t_base = p.row_planes ? 0 : (tc.tti * p.TT + p.t_first) * p.sT - p.pT;
-      const int n_base = tc.nt * BN;
-      // the live groups of the tile: for each live (kt, kh), a run of lv.w.n * kchunks consecutive schedule entries
-      // (kw, then the channel chunk innermost).  j walks them; at the end of a run it jumps over the dead kw taps to the
-      // next live kh row, and after the last live row of a kt plane over the dead kh rows as well.
-      const LiveTaps lv = tile_live(p, tc);
-      const int run = lv.w.n * p.kchunks;
-      const int live = lv.t.n * lv.h.n * run;
-      const int skip_h = (p.kW - lv.w.n) * p.kchunks;
-      const int skip_t = skip_h + (p.kH - lv.h.n) * p.kW * p.kchunks;
-      int j = ((lv.t.k0 * p.kH + lv.h.k0) * p.kW + lv.w.k0) * p.kchunks;
-      int run_end = j + run, rows = lv.h.n;
-      for (int ki = 0; ki < live; ki += KS) {
-        const int nk = min(KS, live - ki);
-        // this stage's groups from the schedule (uniform loads), then ONE elected issue block
-        int jq[2];
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          jq[q] = q < nk ? j : jq[0];                  // an unused second slot re-reads the first entry (never issued)
-          if (q < nk && ++j == run_end) {
-            if (--rows == 0) { rows = lv.h.n; j += skip_t; } else { j += skip_h; }
-            run_end = j + run;
-          }
-        }
-        int x0[2], x1[2], x2[2], x3[2];
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          if (load_b) {
-            const int2 e = tabB[jq[q]];
-            x0[q] = e.x; x1[q] = n_base; x2[q] = e.y; x3[q] = 0;
-          } else {
-            const int4 e = tabA[jq[q]];
-            x0[q] = e.x; x1[q] = w_base + e.y; x2[q] = h_base + e.z; x3[q] = t_base + e.w;
-          }
-        }
-        mbar_wait_u(empty_u + stage * 8, phase ^ 1);
-        if (elect_one()) {
-          const uint32_t bar = full_u + stage * 8;
-          const uint32_t dst = smem_u + stage * stage_bytes;
-          mbar_expect_tx_u(bar, (uint32_t)(nk * nbox) * box_tx);
+  if (warp < EPI_WARP0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+    if (warp == 0 || warp == B_WARP) {
+      // ===================== TMA producers =====================
+      // Two warps: warp 0 loads the activation tiles (and the residual ring), warp B_WARP the weight tiles; both
+      // arm the same full[] barrier with their own byte count, so the scalar bookkeeping of the two operands runs
+      // in parallel.  The whole warp runs the loop (warp-uniform control flow and addresses, so descriptors /
+      // coordinates stay in uniform registers); one elected lane issues.
+      const bool load_b = warp != 0;
+      int stage = 0; uint32_t phase = 0;
+      int rslot = 0; uint32_t rphase = 0;
+      const uint32_t smem_u = smem_u32(smem) + (load_b ? (uint32_t)(NA * Cfg::A_BYTES) : 0u);
+      const uint32_t full_u = smem_u32(full), empty_u = smem_u32(empty);
+      const int KS = p.ks;                                  // groups per ring stage (one mbarrier round trip)
+      const int nbox = load_b ? NB : NA;                    // this warp's boxes per group: hi, then lo
+      const uint32_t box_bytes = load_b ? (uint32_t)Cfg::B_BYTES : (uint32_t)Cfg::A_BYTES;
+      const uint32_t box_tx = load_b ? (uint32_t)Cfg::B_BYTES : p.a_bytes;
+      const int lo_c = load_b ? p.b_lo_off : p.a_lo_off;    // the lo box: channel offset / weight block offset
+      const int lo_blk = load_b ? p.b_lo_blk : 0;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        const TileCoord tc = decode_tile(p, tile);
+        const int n = tc.tbi * p.TB;
+        const int w_base = tc.twi * p.TW * p.sW - p.pW;
+        const int h_base = tc.thi * p.TH * p.sH - p.pH;
+        const int t_base = p.row_planes ? 0 : (tc.tti * p.TT + p.t_first) * p.sT - p.pT;
+        const int n_base = tc.nt * BN;
+        // the live groups of the tile: for each live (kt, kh), a run of lv.w.n * kchunks consecutive schedule entries
+        // (kw, then the channel chunk innermost).  j walks them; at the end of a run it jumps over the dead kw taps to the
+        // next live kh row, and after the last live row of a kt plane over the dead kh rows as well.
+        const LiveTaps lv = tile_live(p, tc);
+        const int run = lv.w.n * p.kchunks;
+        const int live = lv.t.n * lv.h.n * run;
+        const int skip_h = (p.kW - lv.w.n) * p.kchunks;
+        const int skip_t = skip_h + (p.kH - lv.h.n) * p.kW * p.kchunks;
+        int j = ((lv.t.k0 * p.kH + lv.h.k0) * p.kW + lv.w.k0) * p.kchunks;
+        int run_end = j + run, rows = lv.h.n;
+        for (int ki = 0; ki < live; ki += KS) {
+          const int nk = min(KS, live - ki);
+          // this stage's groups from the schedule (uniform loads), then ONE elected issue block
+          int jq[2];
 #pragma unroll
           for (int q = 0; q < 2; ++q) {
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              if (q >= nk || i >= nbox) continue;
-              const uint32_t d = dst + q * group_bytes + i * box_bytes;
-              if (load_b) tma_load_3d_u(d, &tmB, bar, x0[q] + i * lo_c, x1[q], x2[q] + i * lo_blk);
-              else tma_load_5d_u(d, &tmA, bar, x0[q] + i * lo_c, x1[q], x2[q], x3[q], n);
+            jq[q] = q < nk ? j : jq[0];                  // an unused second slot re-reads the first entry (never issued)
+            if (q < nk && ++j == run_end) {
+              if (--rows == 0) { rows = lv.h.n; j += skip_t; } else { j += skip_h; }
+              run_end = j + run;
             }
           }
-        }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (p.nrbuf > 0 && !load_b) {
-        // residual chunks of this tile (bf16, same box as the output chunks), consumed in order by the epilogue
-        const int ncols = min(BN, p.Cout - n_base);
-        for (int cc = 0; cc < ncols; cc += 64) {
-          mbar_wait(&r_empty[rslot], rphase ^ 1);
-          if (elect_one()) {
-            const uint32_t bar = smem_u32(&r_full[rslot]);
-            const uint32_t rbytes = p.res_up ? p.a_bytes >> 2 : p.a_bytes;
-            mbar_expect_tx_u(bar, SPLIT ? 2u * rbytes : rbytes);
-            tma_load_5d_u(smem_u32(rbuf) + rslot * rslot_bytes, &tmR, bar, n_base + cc, (tc.twi * p.TW) >> p.res_up,
-                          (tc.thi * p.TH) >> p.res_up, tc.tti * p.TT, n);
-            if (SPLIT)
-              tma_load_5d_u(smem_u32(rbuf) + rslot * rslot_bytes + Cfg::C_BYTES, &tmR, bar, n_base + cc + p.res_lo_off,
-                            (tc.twi * p.TW) >> p.res_up, (tc.thi * p.TH) >> p.res_up, tc.tti * p.TT, n);
+          int x0[2], x1[2], x2[2], x3[2];
+#pragma unroll
+          for (int q = 0; q < 2; ++q) {
+            if (load_b) {
+              const int2 e = tabB[jq[q]];
+              x0[q] = e.x; x1[q] = n_base; x2[q] = e.y; x3[q] = 0;
+            } else {
+              const int4 e = tabA[jq[q]];
+              x0[q] = e.x; x1[q] = w_base + e.y; x2[q] = h_base + e.z; x3[q] = t_base + e.w;
+            }
           }
-          if (++rslot == p.nrbuf) { rslot = 0; rphase ^= 1; }
+          mbar_wait_u(empty_u + stage * 8, phase ^ 1);
+          if (elect_one()) {
+            const uint32_t bar = full_u + stage * 8;
+            const uint32_t dst = smem_u + stage * stage_bytes;
+            mbar_expect_tx_u(bar, (uint32_t)(nk * nbox) * box_tx);
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                if (q >= nk || i >= nbox) continue;
+                const uint32_t d = dst + q * group_bytes + i * box_bytes;
+                if (load_b) tma_load_3d_u(d, &tmB, bar, x0[q] + i * lo_c, x1[q], x2[q] + i * lo_blk);
+                else tma_load_5d_u(d, &tmA, bar, x0[q] + i * lo_c, x1[q], x2[q], x3[q], n);
+              }
+            }
+          }
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        if (RES == RES_TMA && !load_b) {
+          // residual chunks of this tile (bf16, same box as the output chunks), consumed in order by the epilogue
+          const int ncols = min(BN, p.Cout - n_base);
+          for (int cc = 0; cc < ncols; cc += 64) {
+            mbar_wait(&r_empty[rslot], rphase ^ 1);
+            if (elect_one()) {
+              const uint32_t bar = smem_u32(&r_full[rslot]);
+              const uint32_t rbytes = p.res_up ? p.a_bytes >> 2 : p.a_bytes;
+              mbar_expect_tx_u(bar, SPLIT ? 2u * rbytes : rbytes);
+              tma_load_5d_u(smem_u32(rbuf) + rslot * rslot_bytes, &tmR, bar, n_base + cc, (tc.twi * p.TW) >> p.res_up,
+                            (tc.thi * p.TH) >> p.res_up, tc.tti * p.TT, n);
+              if (SPLIT)
+                tma_load_5d_u(smem_u32(rbuf) + rslot * rslot_bytes + Cfg::C_BYTES, &tmR, bar, n_base + cc + p.res_lo_off,
+                              (tc.twi * p.TW) >> p.res_up, (tc.thi * p.TH) >> p.res_up, tc.tti * p.TT, n);
+            }
+            if (++rslot == p.nrbuf) { rslot = 0; rphase ^= 1; }
+          }
         }
       }
-    }
-  } else if (warp == 2) {
-    // ===================== TMA store warp =====================
-    // Waits until all epilogue warps have staged a chunk (c_full), stores it (one elected lane, which also owns
-    // the bulk async-groups) and hands staging slots back (c_free) once their store has read them out.  Keeping
-    // this off the epilogue warps removes every block-wide barrier from the epilogue.
-    constexpr bool split_out = SPLIT;
-    const int CW = p.out_f32 ? 32 : 64;
-    const int nslots = split_out ? p.ncbuf / 2 : p.ncbuf;     // split output: a slot is a (hi, lo) buffer pair
-    const uint32_t slot_bytes = split_out ? 2u * Cfg::C_BYTES : (uint32_t)Cfg::C_BYTES;
-    const uint32_t cbuf_u32 = smem_u32(cbuf);
-    int slot = 0, prev_slot = 0; uint32_t sphase = 0;
-    int issued = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const TileCoord tc = decode_tile(p, tile);
-      const int nbase = tc.nt * BN;
-      const int ncols = min(BN, p.Cout - nbase);
-      const int cw0 = tc.twi * p.TW, ch0 = tc.thi * p.TH, ct0 = tc.tti * p.TT, cn0 = tc.tbi * p.TB;
-      for (int cc = 0; cc < ncols; cc += CW) {
-        mbar_wait(&c_full[slot], sphase);
-        if (elect_one()) {
-          const uint32_t buf = cbuf_u32 + (uint32_t)slot * slot_bytes;
-          tma_store_5d(&tmC, buf, nbase + cc, cw0, ch0, ct0, cn0);
-          if (split_out) tma_store_5d(&tmC, buf + Cfg::C_BYTES, nbase + cc + p.out_lo_off, cw0, ch0, ct0, cn0);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    } else if (warp == 2) {
+      // ===================== TMA store warp =====================
+      // Waits until the warps of the tile's warpgroup have staged a chunk (c_full), stores it (one elected lane, which owns
+      // the bulk async-groups too) and hands staging slots back (c_free) once their store has read them out.  Keeping
+      // this off the epilogue warps removes every block-wide barrier from the epilogue.
+      constexpr bool split_out = SPLIT;
+      constexpr int CW = OUT_F32 ? 32 : 64;
+      const int nslots = split_out ? p.ncbuf / 2 : p.ncbuf;     // split output: a slot is a (hi, lo) buffer pair
+      const uint32_t slot_bytes = split_out ? 2u * Cfg::C_BYTES : (uint32_t)Cfg::C_BYTES;
+      const uint32_t cbuf_u32 = smem_u32(cbuf);
+      int slot = 0, prev_slot = 0; uint32_t sphase = 0;
+      int issued = 0;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        const TileCoord tc = decode_tile(p, tile);
+        const int nbase = tc.nt * BN;
+        const int ncols = min(BN, p.Cout - nbase);
+        const int cw0 = tc.twi * p.TW, ch0 = tc.thi * p.TH, ct0 = tc.tti * p.TT, cn0 = tc.tbi * p.TB;
+        for (int cc = 0; cc < ncols; cc += CW) {
+          mbar_wait(&c_full[slot], sphase);
+          if (elect_one()) {
+            const uint32_t buf = cbuf_u32 + (uint32_t)slot * slot_bytes;
+            tma_store_5d(&tmC, buf, nbase + cc, cw0, ch0, ct0, cn0);
+            if (split_out) tma_store_5d(&tmC, buf + Cfg::C_BYTES, nbase + cc + p.out_lo_off, cw0, ch0, ct0, cn0);
+            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+          }
+          // hand back the slot of the PREVIOUS chunk as soon as its store has read it out (at most this chunk's
+          // store stays pending), so the epilogue warps may run nslots - 1 chunks ahead of the slowest one
+          if (nslots == 1) {
+            if (elect_one()) { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); mbar_arrive(&c_free[0]); }
+          } else if (issued > 0) {
+            if (elect_one()) { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); mbar_arrive(&c_free[prev_slot]); }
+          }
+          prev_slot = slot;
+          ++issued;
+          if (++slot == nslots) { slot = 0; sphase ^= 1; }
+          __syncwarp();
         }
-        // hand back the slot of the PREVIOUS chunk as soon as its store has read it out (at most this chunk's
-        // store stays pending), so the epilogue warps may run nslots - 1 chunks ahead of the slowest one
-        if (nslots == 1) {
-          if (elect_one()) { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); mbar_arrive(&c_free[0]); }
-        } else if (issued > 0) {
-          if (elect_one()) { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); mbar_arrive(&c_free[prev_slot]); }
-        }
-        prev_slot = slot;
-        ++issued;
-        if (++slot == nslots) { slot = 0; sphase ^= 1; }
-        __syncwarp();
       }
+      if (elect_one()) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
     }
-    if (elect_one()) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  } else if (warp >= EPI_WARP0) {
+  } else {
     // ===================== consumers (warps 4..11): wgmma, then the epilogue =====================
-    // Warpgroup g computes rows 64g .. 64g+63 of the tile.  Thread (warp q of its group, lane l) holds the accumulators
-    // of rows 16q + l/4 and 16q + l/4 + 8 of that half, columns 8j + 2(l%4) + {0, 1} (wgmma.cuh).  The epilogue turns
-    // each (row, column pair) into one 4-byte (bf16) / 8-byte (fp32) store into a 128B-swizzled staging chunk (the
-    // eight rows of a warp hit eight different 16-byte units: conflict-free), which the store warp writes out by TMA.
-    // The TMA store writes whole 128-byte lines and clips rows / channels outside the tensor, so ragged tiles need
-    // no predication on the store side.
+    // Ping-pong: warpgroup g runs the tiles k = g, g + 2, g + 4, ... of the CTA's sequence, each whole: per k-step one
+    // m64 wgmma on rows 0-63 into acc[0] and one on rows 64-127 into acc[1], so every output element sees the same
+    // accumulation sequence as with one 64-row half per warpgroup.  While one warpgroup runs a tile's epilogue the other
+    // issues the next tile's MMAs.  Both walk the one operand ring, the staging slots and the residual ring in tile
+    // order and step over what the other's tiles use.  Two order barriers keep the walks in order: a mainloop starts
+    // once the previous tile's mainloop has waited on all its ring stages (ml_ord), so a parity wait never runs a lap
+    // ahead of the ring, and an epilogue starts once the previous tile's epilogue has staged all its chunks (ep_ord).
+    // Thread (warp q of its group, lane l) holds the accumulators of rows 64h + 16q + l/4 and 64h + 16q + l/4 + 8 of
+    // half h, columns 8j + 2(l%4) + {0, 1} (wgmma.cuh).  The epilogue turns each (row, column pair) into one 4-byte
+    // (bf16) / 8-byte (fp32) store into a 128B-swizzled staging chunk (the eight rows of a warp hit eight different
+    // 16-byte units: conflict-free), which the store warp writes out by TMA.  The TMA store writes whole 128-byte lines
+    // and clips rows / channels outside the tensor, so ragged tiles need no predication on the store side.
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
     const int wg = (warp - EPI_WARP0) >> 2;
-    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: row0 and row0 + 8
+    const int row0 = (warp & 3) * 16 + (lane >> 2);   // this thread's rows: 64 (i >> 1) + row0 + 8 (i & 1), i = 0..3
     const int cq = lane & 3;
-    const bool out_f32 = p.out_f32 != 0;
+    constexpr bool out_f32 = OUT_F32;
     constexpr bool split_out = SPLIT;
     const bool relu = p.relu != 0;
     const int res_mode = p.res_mode;
     const int Cout = p.Cout;
-    const int JPC = out_f32 ? 4 : 8;           // 8-column accumulator groups per 128-byte staged chunk
+    constexpr int JPC = out_f32 ? 4 : 8;       // 8-column accumulator groups per 128-byte staged chunk
+    constexpr int JB = out_f32 && !split_out ? 2 : 1;   // groups whose residual loads are issued together (registers)
     const int nslots = split_out ? p.ncbuf / 2 : p.ncbuf;
     const uint32_t slot_bytes = split_out ? 2u * Cfg::C_BYTES : (uint32_t)Cfg::C_BYTES;
     const uint32_t cbuf_u32 = smem_u32(cbuf);
     const uint32_t rbuf_u32 = smem_u32(rbuf);
-    const bool res_tma = p.nrbuf > 0;
-    const bool res_ldg = res_mode != 0 && !res_tma;
-    // per row i: position inside the tile, staging row offset and swizzle, residual ring row (top-down add: the row of
-    // its parent position in the (TH/2 x TW/2) box of the coarser map)
-    int tw_[2], th_[2], tl_[2], nl_[2];
-    uint32_t srow[2], sswz[2], rrow[2], rswz[2];
+    constexpr bool res_tma = RES == RES_TMA;
+    constexpr bool res_ldg = RES == RES_LDG;
+    // row i of this thread: tile row 64 (i >> 1) + row0 + 8 (i & 1), staged at that row (its swizzle, row & 7, is the
+    // same for all four rows); its position inside the tile (tw, th, tl, nl) is decoded where needed rather than kept
+    // in registers across the tile loop.  rrow: its residual ring row (top-down add: the row of its parent position in
+    // the (TH/2 x TW/2) box of the coarser map)
+    const uint32_t sswz = (uint32_t)(row0 & 7);
+    struct RowPos { int tw, th, tl, nl; };
+    auto row_pos = [&](int i) {
+      int rr = 64 * (i >> 1) + row0 + 8 * (i & 1);
+      RowPos r;
+      r.tw = rr % p.TW; rr /= p.TW;
+      r.th = rr % p.TH; rr /= p.TH;
+      r.tl = rr % p.TT;
+      r.nl = rr / p.TT;                        // >= TB for the unused tail rows of a short tile
+      return r;
+    };
+    uint32_t rrow[4];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      int rr = row0 + 8 * i;
-      srow[i] = (uint32_t)rr * 128u; sswz[i] = (uint32_t)(rr & 7);
-      tw_[i] = rr % p.TW; rr /= p.TW;
-      th_[i] = rr % p.TH; rr /= p.TH;
-      tl_[i] = rr % p.TT;
-      nl_[i] = rr / p.TT;                      // >= TB for the unused tail rows of a short tile
-      const int rp = p.res_up ? ((nl_[i] * p.TT + tl_[i]) * (p.TH >> 1) + (th_[i] >> 1)) * (p.TW >> 1) + (tw_[i] >> 1)
-                              : row0 + 8 * i;
-      rrow[i] = (uint32_t)rp * 128u; rswz[i] = (uint32_t)(rp & 7);
+    for (int i = 0; i < 4; ++i) {
+      int rp = 64 * (i >> 1) + row0 + 8 * (i & 1);
+      if (p.res_up) {
+        const RowPos r = row_pos(i);
+        rp = ((r.nl * p.TT + r.tl) * (p.TH >> 1) + (r.th >> 1)) * (p.TW >> 1) + (r.tw >> 1);
+      }
+      rrow[i] = (uint32_t)rp * 128u;
     }
     const float* __restrict__ g_scale = p.scale;
     const float* __restrict__ g_bias = p.bias;
-    const uint32_t smem_u = smem_u32(smem) + (uint32_t)wg * (64u * 128u);   // this warpgroup's 64 rows of the A tile
+    const uint32_t smem_u = smem_u32(smem);
     const uint32_t full_u = smem_u32(full);
     const int KS = p.ks;
     int stage = 0; uint32_t phase = 0;
     int rslot = 0; uint32_t rphase = 0;
     int slot = 0; uint32_t sphase = 0;
-    float acc[BN / 2];
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    uint32_t ml_par = 0, ep_par = 0;           // parities of the next waits on the other warpgroup's order barriers
+    float acc[2][BN / 2];
+    int k = 0;                                 // position of the tile in the CTA's sequence
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++k) {
       const TileCoord tc = decode_tile(p, tile);
+      const LiveTaps lv = tile_live(p, tc);
+      const int live = lv.t.n * lv.h.n * lv.w.n * p.kchunks;
+      const int nbase = tc.nt * BN;
+      const int ncols = min(BN, Cout - nbase);     // live output columns of this tile
+      if ((k & 1) != wg) {
+        // the other warpgroup's tile: step over its ring stages (one per KS live groups; none when no group is live),
+        // its staged chunks and its residual chunks (one per chunk)
+        stage += (live + KS - 1) / KS; phase ^= (uint32_t)(stage / STAGES) & 1u; stage %= STAGES;
+        const int nch = (ncols + 8 * JPC - 1) / (8 * JPC);
+        slot += nch; sphase ^= (uint32_t)(slot / nslots) & 1u; slot %= nslots;
+        if (res_tma) { rslot += nch; rphase ^= (uint32_t)(rslot / p.nrbuf) & 1u; rslot %= p.nrbuf; }
+        continue;
+      }
+      if (k > 0) { mbar_wait(&ml_ord[wg ^ 1], ml_par); ml_par ^= 1u; }
       // ---- main loop: one wgmma group per (tap, channel chunk) group; a ring stage goes back to the producers once
       // the wgmma group of the NEXT stage's last group is issued and the stage's own wgmma groups retired (one stage
       // stays in flight).  The wgmmas sit outside any branch so that they are not serialized.
       // only the tile's live groups are issued (the producers walk the same ones, tile_live); ki, and with it the
       // pairing into ring stages and scale-d of the first wgmma, counts from the first live group
-      const LiveTaps lv = tile_live(p, tc);
-      const int live = lv.t.n * lv.h.n * lv.w.n * p.kchunks;
       if (live == 0) {
         // no live group (every box of the tile lies in the zero padding, e.g. a 1x1x1 conv with temporal padding on its
         // first / last frame): the conv is 0 and no ring stage is used.  The epilogue still runs on that (scale * 0 +
         // bias, residual, ReLU), not on the previous tile's accumulators
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int i = 0; i < BN / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
       }
       int prev = -1;
       for (int ki = 0; ki < live; ++ki) {
@@ -476,11 +528,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           // products in a fixed order: A_0 W_0, then A_1 W_0 (split), then A_0 W_1 (split, split conv1)
           const uint32_t ai = (NA == 2 && s == 1) ? 1u : 0u;
           const uint32_t bi = (NB == 2 && s == NMMA - 1) ? 1u : 0u;
-          const uint64_t adesc = make_sw128_desc(smem_u + off + ai * Cfg::A_BYTES);
-          const uint64_t bdesc = make_sw128_desc(smem_u32(smem) + off + NA * Cfg::A_BYTES + bi * Cfg::B_BYTES);
+          const uint64_t adesc0 = make_sw128_desc(smem_u + off + ai * Cfg::A_BYTES);
+          const uint64_t adesc1 = make_sw128_desc(smem_u + off + ai * Cfg::A_BYTES + 64u * 128u);   // rows 64-127
+          const uint64_t bdesc = make_sw128_desc(smem_u + off + NA * Cfg::A_BYTES + bi * Cfg::B_BYTES);
 #pragma unroll
-          for (int k = 0; k < 4; ++k)                  // 4 x 32 B = one 128-byte swizzle row of K
-            wgmma<BN, KIND>(acc, adesc + 2 * k, bdesc + 2 * k, (ki | s | k) != 0 ? 1u : 0u);
+          for (int kk = 0; kk < 4; ++kk) {             // 4 x 32 B = one 128-byte swizzle row of K
+            const uint32_t sd = (ki | s | kk) != 0 ? 1u : 0u;
+            wgmma<BN, KIND>(acc[0], adesc0 + 2 * kk, bdesc + 2 * kk, sd);
+            wgmma<BN, KIND>(acc[1], adesc1 + 2 * kk, bdesc + 2 * kk, sd);
+          }
         }
         wgmma_commit();
         if (q == KS - 1 || ki == live - 1) {
@@ -490,123 +546,170 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
+      // every ring stage of this tile has been waited on: the other warpgroup may start the next tile's mainloop
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&ml_ord[wg]);
       wgmma_wait<0>();
       __syncwarp();
       if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
 
+      if (k > 0) { mbar_wait(&ep_ord[wg ^ 1], ep_par); ep_par ^= 1u; }
+
       // ---- epilogue
-      bool valid[2] = {true, true};
-      size_t rpos[2] = {0, 0};
+      long long rpos[4] = {-1, -1, -1, -1};    // residual position of row i, -1 outside the output
       if (res_ldg) {                           // per-thread residual rows (fp32 / upsample-add paths only)
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int ho = tc.thi * p.TH + th_[i], wo = tc.twi * p.TW + tw_[i];
-          const int t = tc.tti * p.TT + tl_[i], n = tc.tbi * p.TB + nl_[i];
-          valid[i] = (nl_[i] < p.TB) && (ho < p.Ho) && (wo < p.Wo) && (t < p.To) && (n < p.N);
-          rpos[i] = (res_mode == 2) ? ((size_t)(n * p.To + t) * (p.Ho >> 1) + (ho >> 1)) * (p.Wo >> 1) + (wo >> 1)
-                                    : ((size_t)(n * p.To + t) * p.Ho + ho) * p.Wo + wo;
+        for (int i = 0; i < 4; ++i) {
+          const RowPos r = row_pos(i);
+          const int ho = tc.thi * p.TH + r.th, wo = tc.twi * p.TW + r.tw;
+          const int t = tc.tti * p.TT + r.tl, n = tc.tbi * p.TB + r.nl;
+          if ((r.nl < p.TB) && (ho < p.Ho) && (wo < p.Wo) && (t < p.To) && (n < p.N))
+            rpos[i] = (res_mode == 2) ? ((long long)(n * p.To + t) * (p.Ho >> 1) + (ho >> 1)) * (p.Wo >> 1) + (wo >> 1)
+                                      : ((long long)(n * p.To + t) * p.Ho + ho) * p.Wo + wo;
         }
       }
-      const int nbase = tc.nt * BN;
-      const int ncols = min(BN, Cout - nbase);     // live output columns of this tile
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        if (8 * j >= ncols) break;
-        const int jc = j % JPC;                    // 8-column group inside the staged chunk
-        const int col = nbase + 8 * j + 2 * cq;    // first of this thread's two output channels
-        if (jc == 0) {
-          // chunk start: the staging slot must have been read out by the TMA store that used it last (c_free), and
-          // the producer's residual chunk must have landed
-          mbar_wait(&c_free[slot], sphase ^ 1);
-          if (res_tma) mbar_wait(&r_full[rslot], rphase);
-        }
-        float sc0 = 1.f, sc1 = 1.f, bi0 = 0.f, bi1 = 0.f;
-        if (col + 2 <= Cout) {
-          if (g_scale) { const float2 s2 = __ldg(reinterpret_cast<const float2*>(g_scale + col)); sc0 = s2.x; sc1 = s2.y; }
-          if (g_bias) { const float2 b2 = __ldg(reinterpret_cast<const float2*>(g_bias + col)); bi0 = b2.x; bi1 = b2.y; }
-        } else if (col < Cout) {                   // ragged channel tail
-          if (g_scale) sc0 = __ldg(g_scale + col);
-          if (g_bias) bi0 = __ldg(g_bias + col);
-        }
+      for (int j0 = 0; j0 < BN / 8; j0 += JPC) {   // one staged chunk: the 8-column groups j0 .. j0 + JPC - 1
+        if (8 * j0 >= ncols) break;
+        // chunk start: the staging slot must have been read out by the TMA store that used it last (c_free), and
+        // the producer's residual chunk must have landed
+        mbar_wait(&c_free[slot], sphase ^ 1);
+        if (res_tma) mbar_wait(&r_full[rslot], rphase);
         const uint32_t dst_slot = cbuf_u32 + (uint32_t)slot * slot_bytes;
         const uint32_t src_slot = rbuf_u32 + (uint32_t)rslot * rslot_bytes;
+        // affine and residual of JB column groups first, then their stores: a store is an ordered memory operation,
+        // so a residual load after it would only start then and the loads' latencies would add up.  fp32 chunks
+        // batch the whole chunk; bf16 chunks (twice the groups) one group, which keeps them within the registers
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          float v0 = fmaf(acc[4 * j + 2 * i], sc0, bi0);
-          float v1 = fmaf(acc[4 * j + 2 * i + 1], sc1, bi1);
-          if (out_f32) {
-            if (res_mode != 0 && valid[i]) {
-              const float* rp = reinterpret_cast<const float*>(p.residual) + rpos[i] * p.res_ld + col;
-              if (col + 2 <= Cout) {
-                const float2 q = __ldg(reinterpret_cast<const float2*>(rp));
-                v0 += q.x; v1 += q.y;
-                if (split_out) {                                     // residual = hi + lo
-                  const float2 ql = __ldg(reinterpret_cast<const float2*>(rp + p.res_lo_off));
-                  v0 += ql.x; v1 += ql.y;
+        for (int jb = 0; jb < JPC; jb += JB) {
+          float v[JB][4][2];
+          // per-thread residual loads (hi, lo) of the JB groups' full column pairs, all issued before the first use
+          float2 rq[JB][4], rl[JB][4];
+          uint32_t rb[JB][4], rbl[JB][4];
+#pragma unroll
+          for (int jc = jb; jc < jb + JB; ++jc) {
+            const int col = nbase + 8 * (j0 + jc) + 2 * cq;
+            if (res_ldg && j0 + jc < BN / 8 && 8 * (j0 + jc) < ncols && col + 2 <= Cout) {
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                if (rpos[i] < 0) continue;
+                if (out_f32) {
+                  const float* rp = reinterpret_cast<const float*>(p.residual) + (size_t)rpos[i] * p.res_ld + col;
+                  rq[jc - jb][i] = __ldg(reinterpret_cast<const float2*>(rp));
+                  if (split_out) rl[jc - jb][i] = __ldg(reinterpret_cast<const float2*>(rp + p.res_lo_off));
+                } else {
+                  const __nv_bfloat16* rp =
+                      reinterpret_cast<const __nv_bfloat16*>(p.residual) + (size_t)rpos[i] * p.res_ld + col;
+                  rb[jc - jb][i] = __ldg(reinterpret_cast<const unsigned int*>(rp));
+                  if (SPLIT) rbl[jc - jb][i] = __ldg(reinterpret_cast<const unsigned int*>(rp + p.res_lo_off));
                 }
-              } else if (col < Cout) {
-                v0 += __ldg(rp) + (split_out ? __ldg(rp + p.res_lo_off) : 0.f);
               }
             }
-            if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-            // 8 bytes at chunk column 8 jc + 2 cq: 16-byte unit 2 jc + cq / 2, offset 8 (cq & 1)
-            const uint32_t off = ((((uint32_t)(2 * jc + (cq >> 1))) ^ sswz[i]) << 4) + 8u * (cq & 1);
-            const uint32_t dst = dst_slot + srow[i] + off;
-            if (split_out) {
-              const float h0 = round_to_tf32(v0), h1 = round_to_tf32(v1);
-              sts_f2(dst + Cfg::C_BYTES, round_to_tf32(v0 - h0), round_to_tf32(v1 - h1));   // lo: the slot's second buffer
-              v0 = h0; v1 = h1;
-            } else if (p.round_tf32) {
-              v0 = round_to_tf32(v0); v1 = round_to_tf32(v1);
+          }
+#pragma unroll
+          for (int jc = jb; jc < jb + JB; ++jc) {
+            const int j = j0 + jc;
+            if (j >= BN / 8 || 8 * j >= ncols) break;
+            const int col = nbase + 8 * j + 2 * cq;  // first of this thread's two output channels
+            float sc0 = 1.f, sc1 = 1.f, bi0 = 0.f, bi1 = 0.f;
+            if (col + 2 <= Cout) {
+              if (g_scale) { const float2 s2 = __ldg(reinterpret_cast<const float2*>(g_scale + col)); sc0 = s2.x; sc1 = s2.y; }
+              if (g_bias) { const float2 b2 = __ldg(reinterpret_cast<const float2*>(g_bias + col)); bi0 = b2.x; bi1 = b2.y; }
+            } else if (col < Cout) {                 // ragged channel tail
+              if (g_scale) sc0 = __ldg(g_scale + col);
+              if (g_bias) bi0 = __ldg(g_bias + col);
             }
-            sts_f2(dst, v0, v1);
-          } else {
-            // 4 bytes at chunk column 8 jc + 2 cq: 16-byte unit jc, offset 4 cq
-            if (res_tma) {
-              const uint32_t src = src_slot + rrow[i] + ((((uint32_t)jc) ^ rswz[i]) << 4) + 4u * cq;
-              uint32_t r2 = lds_b1(src);
-              v0 += __uint_as_float(r2 << 16); v1 += __uint_as_float(r2 & 0xffff0000u);
-              if (SPLIT) { r2 = lds_b1(src + Cfg::C_BYTES); v0 += __uint_as_float(r2 << 16); v1 += __uint_as_float(r2 & 0xffff0000u); }
-            } else if (res_ldg && valid[i]) {
-              const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.residual) + rpos[i] * p.res_ld + col;
-              if (col + 2 <= Cout) {
-                uint32_t r2 = __ldg(reinterpret_cast<const unsigned int*>(rp));
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              float v0 = fmaf(acc[i >> 1][4 * j + 2 * (i & 1)], sc0, bi0);
+              float v1 = fmaf(acc[i >> 1][4 * j + 2 * (i & 1) + 1], sc1, bi1);
+              if (out_f32) {
+                if (res_ldg && rpos[i] >= 0) {
+                  const float* rp = reinterpret_cast<const float*>(p.residual) + (size_t)rpos[i] * p.res_ld + col;
+                  if (col + 2 <= Cout) {
+                    const float2 q = rq[jc - jb][i];
+                    v0 += q.x; v1 += q.y;
+                    if (split_out) {                                     // residual = hi + lo
+                      const float2 ql = rl[jc - jb][i];
+                      v0 += ql.x; v1 += ql.y;
+                    }
+                  } else if (col < Cout) {
+                    v0 += __ldg(rp) + (split_out ? __ldg(rp + p.res_lo_off) : 0.f);
+                  }
+                }
+              } else if (res_tma) {
+                const uint32_t src = src_slot + rrow[i] + ((((uint32_t)jc) ^ ((rrow[i] >> 7) & 7u)) << 4) + 4u * cq;
+                uint32_t r2 = lds_b1(src);
                 v0 += __uint_as_float(r2 << 16); v1 += __uint_as_float(r2 & 0xffff0000u);
-                if (SPLIT) {                                          // residual = hi + lo (bf16 pairs)
-                  r2 = __ldg(reinterpret_cast<const unsigned int*>(rp + p.res_lo_off));
+                if (SPLIT) { r2 = lds_b1(src + Cfg::C_BYTES); v0 += __uint_as_float(r2 << 16); v1 += __uint_as_float(r2 & 0xffff0000u); }
+              } else if (res_ldg && rpos[i] >= 0) {
+                const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.residual) + (size_t)rpos[i] * p.res_ld + col;
+                if (col + 2 <= Cout) {
+                  uint32_t r2 = rb[jc - jb][i];
                   v0 += __uint_as_float(r2 << 16); v1 += __uint_as_float(r2 & 0xffff0000u);
+                  if (SPLIT) {                                          // residual = hi + lo (bf16 pairs)
+                    r2 = rbl[jc - jb][i];
+                    v0 += __uint_as_float(r2 << 16); v1 += __uint_as_float(r2 & 0xffff0000u);
+                  }
+                } else if (col < Cout) {
+                  v0 += __bfloat162float(rp[0]) + (SPLIT ? __bfloat162float(rp[p.res_lo_off]) : 0.f);
                 }
-              } else if (col < Cout) {
-                v0 += __bfloat162float(rp[0]) + (SPLIT ? __bfloat162float(rp[p.res_lo_off]) : 0.f);
+              }
+              v[jc - jb][i][0] = v0; v[jc - jb][i][1] = v1;
+            }
+          }
+#pragma unroll
+          for (int jc = jb; jc < jb + JB; ++jc) {
+            if (j0 + jc >= BN / 8 || 8 * (j0 + jc) >= ncols) break;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              float v0 = v[jc - jb][i][0], v1 = v[jc - jb][i][1];
+              const uint32_t row_off = (uint32_t)(64 * (i >> 1) + row0 + 8 * (i & 1)) * 128u;
+              if (out_f32) {
+                if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                // 8 bytes at chunk column 8 jc + 2 cq: 16-byte unit 2 jc + cq / 2, offset 8 (cq & 1)
+                const uint32_t off = ((((uint32_t)(2 * jc + (cq >> 1))) ^ sswz) << 4) + 8u * (cq & 1);
+                const uint32_t dst = dst_slot + row_off + off;
+                if (split_out) {
+                  const float h0 = round_to_tf32(v0), h1 = round_to_tf32(v1);
+                  sts_f2(dst + Cfg::C_BYTES, round_to_tf32(v0 - h0), round_to_tf32(v1 - h1));   // lo: the slot's second buffer
+                  v0 = h0; v1 = h1;
+                } else if (p.round_tf32) {
+                  v0 = round_to_tf32(v0); v1 = round_to_tf32(v1);
+                }
+                sts_f2(dst, v0, v1);
+              } else {
+                // 4 bytes at chunk column 8 jc + 2 cq: 16-byte unit jc, offset 4 cq
+                const uint32_t dst = dst_slot + row_off + ((((uint32_t)jc) ^ sswz) << 4) + 4u * cq;
+                if (split_out) {
+                  // bf16 pair storage: hi = bf16(v), lo = bf16(v - hi) (v - hi is exact in fp32); hi + lo carries 16
+                  // mantissa bits, which three bf16 MMAs per k-block turn into an fp32-accurate product
+                  if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                  const uint32_t h = pack_bf16x2(v0, v1);
+                  sts_b1(dst + Cfg::C_BYTES, pack_bf16x2(v0 - __uint_as_float(h << 16), v1 - __uint_as_float(h & 0xffff0000u)));
+                  sts_b1(dst, h);
+                } else {
+                  sts_b1(dst, relu ? pack_bf16x2_relu(v0, v1) : pack_bf16x2(v0, v1));
+                }
               }
             }
-            const uint32_t dst = dst_slot + srow[i] + ((((uint32_t)jc) ^ sswz[i]) << 4) + 4u * cq;
-            if (split_out) {
-              // bf16 pair storage: hi = bf16(v), lo = bf16(v - hi) (v - hi is exact in fp32); hi + lo carries 16
-              // mantissa bits, which three bf16 MMAs per k-block turn into an fp32-accurate product
-              if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-              const uint32_t h = pack_bf16x2(v0, v1);
-              sts_b1(dst + Cfg::C_BYTES, pack_bf16x2(v0 - __uint_as_float(h << 16), v1 - __uint_as_float(h & 0xffff0000u)));
-              sts_b1(dst, h);
-            } else {
-              sts_b1(dst, relu ? pack_bf16x2_relu(v0, v1) : pack_bf16x2(v0, v1));
-            }
           }
         }
-        if (jc == JPC - 1 || 8 * (j + 1) >= ncols) {
-          // chunk complete: hand the residual slot back, then generic-proxy smem writes -> visible to the async
-          // proxy, then this warp's arrival on the staging slot
-          if (res_tma) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&r_empty[rslot]);
-            if (++rslot == p.nrbuf) { rslot = 0; rphase ^= 1; }
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        // chunk complete: hand the residual slot back, then generic-proxy smem writes -> visible to the async proxy,
+        // then this warp's arrival on the staging slot
+        if (res_tma) {
           __syncwarp();
-          if (lane == 0) mbar_arrive(&c_full[slot]);
-          if (++slot == nslots) { slot = 0; sphase ^= 1; }
+          if (lane == 0) mbar_arrive(&r_empty[rslot]);
+          if (++rslot == p.nrbuf) { rslot = 0; rphase ^= 1; }
         }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&c_full[slot]);
+        if (++slot == nslots) { slot = 0; sphase ^= 1; }
       }
+      // every chunk of this tile is staged (this warp's last c_full arrival is above): the other warpgroup may stage
+      // the next tile's
+      if (lane == 0) mbar_arrive(&ep_ord[wg]);
     }
   }
 }
@@ -714,12 +817,12 @@ static double conv_mma_kblocks(const dt_conv_desc* d, const ConvGeom& g) {
   return (double)g.nmma * g.kchunks * cdiv(d->Cout, g.BN) * cdiv(d->N, ts.tb) * st * sh * sw;
 }
 
-template <int BN, int KIND, bool SPLIT, int NMMA>
-static int launch_conv1(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
-                       const ConvKernelParams& p, int grid, cudaStream_t stream) {
+template <int BN, int KIND, bool SPLIT, int NMMA, bool OUT_F32, int RES>
+static int launch_conv0(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
+                        const ConvKernelParams& p, int grid, cudaStream_t stream) {
   using Cfg = ConvCfg<BN>;
   static DynSmemGrant grant;
-  DT_CHECK_CUDA(grant_dyn_smem(conv_tc_kernel<BN, KIND, SPLIT, NMMA>, Cfg::BUDGET, &grant));
+  DT_CHECK_CUDA(grant_dyn_smem(conv_tc_kernel<BN, KIND, SPLIT, NMMA, OUT_F32, RES>, Cfg::BUDGET, &grant));
   ConvKernelParams q = p;
   const int groups = p.kT * p.kH * p.kW * p.kchunks;
   DT_CHECK_ARG(groups <= 2048, "conv: %d (tap, channel chunk) groups per tile exceed the schedule table", groups);
@@ -738,8 +841,35 @@ static int launch_conv1(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = at; lc.numAttrs = pdl ? 1 : 0;
-  DT_CHECK_CUDA(cudaLaunchKernelEx(&lc, conv_tc_kernel<BN, KIND, SPLIT, NMMA>, tmA, tmB, tmC, tmR, q));
+  DT_CHECK_CUDA(cudaLaunchKernelEx(&lc, conv_tc_kernel<BN, KIND, SPLIT, NMMA, OUT_F32, RES>, tmA, tmB, tmC, tmR, q));
   return 0;
+}
+
+// the epilogue path of the launch: output type and residual kind.  Only the combinations dt_conv3d / dt_conv1_7x7s2 can
+// produce are compiled: the TMA residual ring is bf16 (bf16 operands and outputs), fp16 operands take no residual, split outputs are bf16 pairs from bf16 / fp16 operands and fp32 pairs from tf32 ones, split conv1 has none.
+template <int BN, int KIND, bool SPLIT, int NMMA>
+static int launch_conv1(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
+                        const ConvKernelParams& p, int grid, cudaStream_t stream) {
+  constexpr bool f32_ok = !(SPLIT && KIND != 2) && NMMA != 2, bf16_ok = !(SPLIT && KIND == 2);
+  constexpr bool tma_ok = KIND == 0 && NMMA != 2, ldg_ok = KIND != 1 && NMMA != 2;
+  const int res = p.nrbuf > 0 ? RES_TMA : (p.res_mode != 0 ? RES_LDG : 0);
+  DT_CHECK_ARG((p.out_f32 ? f32_ok : bf16_ok) && (res != RES_TMA || (tma_ok && !p.out_f32)) && (res != RES_LDG || ldg_ok),
+               "conv: no kernel for output f32=%d with residual kind %d", p.out_f32, res);
+  if constexpr (f32_ok) {
+    if (p.out_f32) {
+      if constexpr (ldg_ok)
+        if (res == RES_LDG) return launch_conv0<BN, KIND, SPLIT, NMMA, true, RES_LDG>(tmA, tmB, tmC, tmR, p, grid, stream);
+      return launch_conv0<BN, KIND, SPLIT, NMMA, true, 0>(tmA, tmB, tmC, tmR, p, grid, stream);
+    }
+  }
+  if constexpr (bf16_ok) {
+    if constexpr (tma_ok)
+      if (res == RES_TMA) return launch_conv0<BN, KIND, SPLIT, NMMA, false, RES_TMA>(tmA, tmB, tmC, tmR, p, grid, stream);
+    if constexpr (ldg_ok)
+      if (res == RES_LDG) return launch_conv0<BN, KIND, SPLIT, NMMA, false, RES_LDG>(tmA, tmB, tmC, tmR, p, grid, stream);
+    return launch_conv0<BN, KIND, SPLIT, NMMA, false, 0>(tmA, tmB, tmC, tmR, p, grid, stream);
+  }
+  return 1;
 }
 
 template <int BN, int KIND, int NMMA>
