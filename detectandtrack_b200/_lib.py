@@ -74,7 +74,13 @@ SIGNATURES = {
 HOST_FUNCS = {'dt_planes_ld': ([_i, _i, _i, _i], C.c_int), 'dt_jpeg_available': ([], C.c_int),
               'dt_wgrad_nhwc_plan': ([_i] * 15 + [C.c_void_p], C.c_int),
               'dt_prep_batch': ([C.POINTER(_p), C.POINTER(_i), C.POINTER(_i), C.POINTER(C.c_double), C.POINTER(_i), C.POINTER(_i),
-                                 C.POINTER(_i), _i, _i, C.POINTER(_f), _i, _i, _i, _i, _i, _i, _i, _p, _p], C.c_int)}
+                                 C.POINTER(_i), _i, _i, C.POINTER(_f), _i, _i, _i, _i, _i, _i, _i, _p, _p], C.c_int),
+              # test-time augmentation kernels: launchers like dt_prep_batch, with their argument-error cases in tests/test_tta.py
+              'dt_aug_merge_dets': ([C.POINTER(_p), C.POINTER(_p), C.POINTER(_i), _i, _i, _i, _i, _p, _i, _p, _p, _p], C.c_int),
+              'dt_aug_scale_rois': ([_p, _i, _i, _i, _p, _i, _i, C.c_double, _p, _p], C.c_int),
+              'dt_keypoint_decode_aug': ([_p, C.c_longlong, _i, _i, _i, _i, C.POINTER(_i), C.POINTER(_i), _i, _p, _i, _p, _i, _i,
+                                          _p, _p, _p], C.c_int)}
+AUG_MAX_VIEWS = 16                  # DT_AUG_MAX_VIEWS of include/dt_b200.h
 PREP_MAX_CLIPS = 16                 # DT_PREP_MAX_CLIPS of include/dt_b200.h
 
 

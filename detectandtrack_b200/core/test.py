@@ -3,8 +3,8 @@
 
 ``im`` is the reference's list of T BGR uint8 frames (HxWx3).  Everything between the H2D copy
 of the frames and the D2H copy of the (<=100) detections runs on the device
-(modeling/engine.py) as ONE captured CUDA graph per batch geometry; test-time augmentation
-(COMPETITION_MODE) is outside the hot path.
+(modeling/engine.py) as ONE captured CUDA graph per batch geometry; with TEST.COMPETITION_MODE that graph runs every
+test-time view of core/tta.view_plan and merges them on the device.
 
 ``ClipPipeline`` is that device step behind the reference's per-clip containers: B clips per graph
 replay, frames staged through pinned host buffers filled by loader threads, the upload of step i+1
@@ -16,6 +16,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
+from . import tta
 from .config import cfg
 from ..utils.timer import Timer
 
@@ -33,12 +34,12 @@ class ClipPipeline(object):
     [T, H, W, 3] with GPU work on ``stream`` (device-side JPEG decode, ops/image_ops.jpeg_decode): no pinned staging, only
     the compressed bytes cross PCIe."""
 
-    def __init__(self, model, B, T, H, W, depth=2, loader_threads=2):
+    def __init__(self, model, B, T, H, W, depth=2, loader_threads=2, plan=None):
         eng = model.engine
         torch = eng.torch
         self.torch, self.eng, self.B, self.T, self.H, self.W, self.depth = torch, eng, B, T, H, W, depth
         self.num_classes = eng.spec.num_classes
-        self.static_in, self.replay = eng.capture(B, T, H, W)
+        self.static_in, self.replay = eng.capture(B, T, H, W, plan=plan)
         out = self.replay()
         torch.cuda.synchronize()
         self.cap = out['dets'].shape[2]
@@ -164,14 +165,17 @@ class ClipPipeline(object):
 
 
 def get_pipeline(model, B, T, H, W):
-    """The model's captured pipeline for a batch geometry (built on first use, a few kept)."""
+    """The model's captured pipeline for a batch geometry (built on first use, a few kept).  With TEST.COMPETITION_MODE
+    its step runs the test-time views of core/tta.view_plan, which rejects what the device path does not run before
+    anything is built."""
+    plan = tta.view_plan(cfg, model.engine.spec, H, W) if cfg.TEST.COMPETITION_MODE else None
     cache = model.__dict__.setdefault('_pipelines', OrderedDict())
-    key = (B, T, H, W)
+    key = (B, T, H, W, plan)
     p = cache.get(key)
     if p is None:
         while len(cache) >= _MAX_PIPELINES:
             cache.popitem(last=False)
-        p = cache[key] = ClipPipeline(model, B, T, H, W)
+        p = cache[key] = ClipPipeline(model, B, T, H, W, plan=plan)
     else:
         cache.move_to_end(key)
     return p
@@ -180,8 +184,6 @@ def get_pipeline(model, B, T, H, W):
 def _check_hot_path(box_proposals):
     if box_proposals is not None:
         raise NotImplementedError('precomputed proposals are not on the hot path (FASTER_RCNN models only)')
-    if cfg.TEST.COMPETITION_MODE:
-        raise NotImplementedError('test-time augmentation (TEST.COMPETITION_MODE) is not on the hot path')
 
 
 def im_detect_all(model, im, box_proposals=None, timers=None):

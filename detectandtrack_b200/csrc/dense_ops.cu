@@ -368,57 +368,47 @@ __device__ __forceinline__ void cubic_coeffs(float x, float* c) {
 #define KD_SW 256   // output columns per strip of the separable cubic resize
 #define KD_RB 256   // output rows per block of precomputed vertical weights
 
-__global__ void __launch_bounds__(256)
-keypoint_decode_kernel(const float* __restrict__ lowres, int ldl, int S, int K, int T,
-                       const float* __restrict__ boxes /*[D, ldb] image coords*/, int ldb,
-                       const int* __restrict__ n_dev, int D, int min_size,
-                       float* __restrict__ heat /*[D, T*K, M, M] or null*/,
-                       float* __restrict__ xy /*[D, 4, T*K]*/) {
-  extern __shared__ float sm[];
-  const int M2 = 2 * S, M = 4 * S;
-  float* low = sm;                 // [M2*M2]  kps_score_lowres for this (d, k)
-  float* map = sm + M2 * M2;       // [M*M]    kps_score
-  __shared__ float s_red[32];
-  __shared__ float s_max;
-  const int d = blockIdx.x, k = blockIdx.y, t = blockIdx.z;
-  const int n = n_dev ? min(*n_dev, D) : D;
-  if (d >= n) return;
-  const int tid = threadIdx.x, nth = blockDim.x;
-  // un-pack the sub-pixel channels of frame t (row d*T + t of the time-in-batch lowres tensor)
-  const float* src = lowres + (size_t)(d * T + t) * S * S * ldl;
-  for (int i = tid; i < M2 * M2; i += nth) {
+// Un-packs joint k of one RoI-frame's sub-pixel low-res row block src [S, S, ldl] into low [2S * 2S].
+__device__ __forceinline__ void kd_unpack(const float* __restrict__ src, int S, int ldl, int K, int k, float* low) {
+  const int M2 = 2 * S;
+  for (int i = threadIdx.x; i < M2 * M2; i += blockDim.x) {
     const int oy = i / M2, ox = i - oy * M2;
     low[i] = src[((size_t)(oy >> 1) * S + (ox >> 1)) * ldl + ((oy & 1) * 2 + (ox & 1)) * K + k];
   }
-  __syncthreads();
-  // bilinear ConvTranspose k=4 s=2 p=1: out[o] = sum_i in[i] * f[o - 2i + 1]
-  for (int i = tid; i < M * M; i += nth) {
-    const int oy = i / M, ox = i - oy * M;
-    const int iy0 = (oy + 1) >> 1, ix0 = (ox + 1) >> 1;          // taps i = iy0 (ky = o-2i+1) and iy0-1 (ky+2)
-    float acc = 0.f;
+}
+
+// bilinear ConvTranspose k=4 s=2 p=1 of the un-packed map at output pixel (oy, ox): out[o] = sum_i in[i] * f[o - 2i + 1]
+__device__ __forceinline__ float kd_upsample_px(const float* low, int M2, int oy, int ox) {
+  const int iy0 = (oy + 1) >> 1, ix0 = (ox + 1) >> 1;          // taps i = iy0 (ky = o-2i+1) and iy0-1 (ky+2)
+  float acc = 0.f;
 #pragma unroll
-    for (int a = 0; a < 2; ++a) {
-      const int iy = iy0 - a, ky = oy - 2 * iy + 1;
-      if (iy < 0 || iy >= M2 || ky < 0 || ky > 3) continue;
-      const float fy = 1.f - fabsf(ky - 1.5f) / 2.f;
+  for (int a = 0; a < 2; ++a) {
+    const int iy = iy0 - a, ky = oy - 2 * iy + 1;
+    if (iy < 0 || iy >= M2 || ky < 0 || ky > 3) continue;
+    const float fy = 1.f - fabsf(ky - 1.5f) / 2.f;
 #pragma unroll
-      for (int bq = 0; bq < 2; ++bq) {
-        const int ix = ix0 - bq, kx = ox - 2 * ix + 1;
-        if (ix < 0 || ix >= M2 || kx < 0 || kx > 3) continue;
-        const float fx = 1.f - fabsf(kx - 1.5f) / 2.f;
-        acc += low[iy * M2 + ix] * (fy * fx);
-      }
+    for (int bq = 0; bq < 2; ++bq) {
+      const int ix = ix0 - bq, kx = ox - 2 * ix + 1;
+      if (ix < 0 || ix >= M2 || kx < 0 || kx > 3) continue;
+      const float fx = 1.f - fabsf(kx - 1.5f) / 2.f;
+      acc += low[iy * M2 + ix] * (fy * fx);
     }
-    map[i] = acc;
-    if (heat) heat[(((size_t)d * T + t) * K + k) * M * M + i] = acc;   // channel t*K + k (model_builder.py:865-868)
   }
-  __syncthreads();
-  // ---- heatmaps_to_keypoints (keypoints.py:94-149) for this (roi, keypoint) ----
+  return acc;
+}
+
+// ---- heatmaps_to_keypoints (keypoints.py:94-149) for one (roi, keypoint) M x M map in shared memory ----
+// Block-wide (every thread calls it); map is followed by the scratch the launchers size.  bx = the RoI's image-space box,
+// o = its xy_preds row [4, KT], col = the output column.
+__device__ __forceinline__ void kd_decode_map(float* map, int M, const float* __restrict__ bx, int min_size, float* o, int KT,
+                                              int col) {
+  __shared__ float s_red[32];
+  __shared__ float s_max;
+  const int tid = threadIdx.x, nth = blockDim.x;
   // cv2.resize(INTER_CUBIC) is separable and cv2 evaluates it in this order too: horizontal pass on
   // the source rows (float), then a 4-tap vertical combination.  Work is done in strips of KD_SW output
   // columns: H-pass of all M source rows into smem, then each thread walks its column top to bottom
   // keeping (max, first argmax, online sum of exp(v - max)).
-  const float* bx = boxes + (size_t)d * ldb + 4 * t;
   const float ofx = bx[0], ofy = bx[1];
   const float bw = fmaxf(bx[2] - bx[0], 1.f), bh = fmaxf(bx[3] - bx[1], 1.f);
   int rw = (int)ceilf(bw), rh = (int)ceilf(bh);
@@ -536,14 +526,84 @@ keypoint_decode_kernel(const float* __restrict__ lowres, int ldl, int S, int K, 
     float tot = 0.f;
     for (int w = 0; w < (nth >> 5); ++w) tot += s_red[w];
     const int x_int = (int)(pos % rw), y_int = (int)(pos / rw);
-    const int KT = K * T, col = t * K + k;
-    float* o = xy + (size_t)d * 4 * KT;
     // keypoints.py:140-145: python floats (fp64) until the store into the fp32 result
     o[0 * KT + col] = (float)((x_int + 0.5) * (double)wcorr + (double)ofx);
     o[1 * KT + col] = (float)((y_int + 0.5) * (double)hcorr + (double)ofy);
     o[2 * KT + col] = mx;
     o[3 * KT + col] = 1.f / tot;           // exp(max - max) / sum
   }
+}
+
+__global__ void __launch_bounds__(256)
+keypoint_decode_kernel(const float* __restrict__ lowres, int ldl, int S, int K, int T,
+                       const float* __restrict__ boxes /*[D, ldb] image coords*/, int ldb,
+                       const int* __restrict__ n_dev, int D, int min_size,
+                       float* __restrict__ heat /*[D, T*K, M, M] or null*/,
+                       float* __restrict__ xy /*[D, 4, T*K]*/) {
+  extern __shared__ float sm[];
+  const int M2 = 2 * S, M = 4 * S;
+  float* low = sm;                 // [M2*M2]  kps_score_lowres for this (d, k)
+  float* map = sm + M2 * M2;       // [M*M]    kps_score
+  const int d = blockIdx.x, k = blockIdx.y, t = blockIdx.z;
+  const int n = n_dev ? min(*n_dev, D) : D;
+  if (d >= n) return;
+  // un-pack the sub-pixel channels of frame t (row d*T + t of the time-in-batch lowres tensor)
+  kd_unpack(lowres + (size_t)(d * T + t) * S * S * ldl, S, ldl, K, k, low);
+  __syncthreads();
+  for (int i = threadIdx.x; i < M * M; i += blockDim.x) {
+    const int oy = i / M, ox = i - oy * M;
+    const float acc = kd_upsample_px(low, M2, oy, ox);
+    map[i] = acc;
+    if (heat) heat[(((size_t)d * T + t) * K + k) * M * M + i] = acc;   // channel t*K + k (model_builder.py:865-868)
+  }
+  __syncthreads();
+  kd_decode_map(map, M, boxes + (size_t)d * ldb + 4 * t, min_size, xy + (size_t)d * 4 * K * T, K * T, t * K + k);
+}
+
+// Test-time augmentation of the keypoint stage (lib/core/test.py:686-747) for 2-D heads: V views' low-res maps of the
+// same RoIs, lowres + v * view_stride = [D, S, S, ldl].  Per (roi, joint): every view's M x M kps_score exactly as
+// keypoint_decode_kernel builds it; a flipped view contributes joint perm[k], mirrored in x (flip_heatmaps,
+// lib/utils/keypoints.py:81-91).  The views are combined in view order — HM_AVG: fp32 running sum, then / V (np.mean over
+// axis 0); HM_MAX: running max (np.amax) — and the combined map is decoded against the original boxes.
+struct KdAugTable {
+  int flip[DT_AUG_MAX_VIEWS];
+  int perm[DT_KD_AUG_MAX_K];
+};
+
+__global__ void __launch_bounds__(256)
+keypoint_decode_aug_kernel(const float* __restrict__ lowres, long long view_stride, int ldl, int S, int K, int V,
+                           const __grid_constant__ KdAugTable tab, int hm_max, const float* __restrict__ boxes, int ldb,
+                           const int* __restrict__ n_dev, int D, int min_size, float* __restrict__ heat /*[D, K, M, M] or null*/,
+                           float* __restrict__ xy /*[D, 4, K]*/) {
+  extern __shared__ float sm[];
+  const int M2 = 2 * S, M = 4 * S;
+  float* low = sm;                 // [M2*M2]  one view's kps_score_lowres for this (d, joint)
+  float* map = sm + M2 * M2;       // [M*M]    the combined kps_score
+  const int d = blockIdx.x, k = blockIdx.y;
+  const int n = n_dev ? min(*n_dev, D) : D;
+  if (d >= n) return;
+  for (int v = 0; v < V; ++v) {
+    const int fl = tab.flip[v];
+    if (v) __syncthreads();                                   // the previous view's low map is consumed
+    kd_unpack(lowres + v * view_stride + (size_t)d * S * S * ldl, S, ldl, K, fl ? tab.perm[k] : k, low);
+    __syncthreads();
+    for (int i = threadIdx.x; i < M * M; i += blockDim.x) {
+      const int oy = i / M, ox = i - oy * M;
+      const float val = kd_upsample_px(low, M2, oy, ox);
+      const int dst = oy * M + (fl ? M - 1 - ox : ox);
+      if (v == 0) map[dst] = val;
+      else if (hm_max) { const float cur = map[dst]; map[dst] = cur >= val ? cur : val; }   // np.maximum(cur, val)
+      else map[dst] = __fadd_rn(map[dst], val);
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < M * M; i += blockDim.x) {
+    const float c = hm_max ? map[i] : __fdiv_rn(map[i], (float)V);
+    map[i] = c;
+    if (heat) heat[((size_t)d * K + k) * M * M + i] = c;
+  }
+  __syncthreads();
+  kd_decode_map(map, M, boxes + (size_t)d * ldb, min_size, xy + (size_t)d * 4 * K, K, k);
 }
 
 // ------------------------------------------------------------------- 3-D box head glue
@@ -830,6 +890,36 @@ extern "C" int dt_keypoint_decode(const float* lowres, int ldl, int S, int K, in
   DT_CHECK_CUDA(grant_dyn_smem(keypoint_decode_kernel, (int)smem, &grant));
   dim3 grid(D, K, T);
   keypoint_decode_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(lowres, ldl, S, K, T, boxes, ldb, n_dev, D, min_size, heatmaps, xy_preds);
+  DT_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int dt_keypoint_decode_aug(const float* lowres, long long view_stride, int ldl, int S, int K, int V, const int* flip,
+                                      const int* perm, int hm_max, const float* boxes, int ldb, const int* n_dev, int D,
+                                      int min_size, float* heatmaps, float* xy_preds, void* stream) {
+  DT_CHECK_ARG(S >= 1 && S <= 32 && K >= 1 && K <= DT_KD_AUG_MAX_K && D >= 0 && ldl >= 4 * K && ldb >= 4,
+               "dt_keypoint_decode_aug: bad shape S=%d K=%d D=%d ldl=%d ldb=%d", S, K, D, ldl, ldb);
+  DT_CHECK_ARG(V >= 1 && V <= DT_AUG_MAX_VIEWS, "dt_keypoint_decode_aug: V=%d views (1..%d)", V, DT_AUG_MAX_VIEWS);
+  DT_CHECK_ARG(view_stride >= (long long)D * S * S * ldl, "dt_keypoint_decode_aug: view_stride %lld < D*S*S*ldl", view_stride);
+  DT_CHECK_ARG(hm_max == 0 || hm_max == 1, "dt_keypoint_decode_aug: hm_max must be 0 or 1");
+  DT_CHECK_ARG(flip && perm, "dt_keypoint_decode_aug: null flip / perm table");
+  KdAugTable tab;
+  memset(&tab, 0, sizeof(tab));
+  for (int v = 0; v < V; ++v) tab.flip[v] = flip[v] != 0;
+  unsigned long long seen = 0;
+  for (int k = 0; k < K; ++k) {
+    DT_CHECK_ARG(perm[k] >= 0 && perm[k] < K && !(seen >> perm[k] & 1ull), "dt_keypoint_decode_aug: perm is not a permutation of 0..K-1");
+    seen |= 1ull << perm[k];
+    tab.perm[k] = perm[k];
+  }
+  if (D == 0) return 0;
+  DT_CHECK_ARG(lowres && boxes && xy_preds, "dt_keypoint_decode_aug: null pointer");
+  const size_t smem = (size_t)(4 * S * S + 16 * S * S + 4 * S * KD_SW) * sizeof(float) + (size_t)(KD_SW + KD_RB) * 20;
+  static DynSmemGrant grant;
+  DT_CHECK_CUDA(grant_dyn_smem(keypoint_decode_aug_kernel, (int)smem, &grant));
+  dim3 grid(D, K);
+  keypoint_decode_aug_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(lowres, view_stride, ldl, S, K, V, tab, hm_max, boxes,
+                                                                        ldb, n_dev, D, min_size, heatmaps, xy_preds);
   DT_CHECK_LAUNCH();
   return 0;
 }

@@ -703,3 +703,89 @@ extern "C" int dt_scale_rois(const float* boxes, int ldb, int n, int ncols, cons
   DT_CHECK_LAUNCH();
   return 0;
 }
+
+// ------------------------------------------------------------------- test-time augmentation (lib/core/test.py:255-414)
+// flip_boxes (lib/utils/boxes.py:275-282) on one 4-column box: x1' = W - x2 - 1, x2' = W - x1 - 1 in numpy's fp32
+// arithmetic (two roundings; this unit is compiled without FMA contraction).
+namespace dt {
+__device__ __forceinline__ float flip_x(float w, float x) { return __fsub_rn(__fsub_rn(w, x), 1.f); }
+
+struct AugMergeTable {
+  const float* dets[DT_AUG_MAX_VIEWS];
+  const int* counts[DT_AUG_MAX_VIEWS];
+  int flip[DT_AUG_MAX_VIEWS];
+};
+
+// One CTA per (image, class - 1): the union of the V views' compacted rows in view order (np.vstack of the views), each
+// flipped view's rows mapped back to the original image.  out [B, C-1, V*R, 5].
+__global__ void aug_merge_dets_kernel(const __grid_constant__ AugMergeTable tab, int V, int ncls1, int R,
+                                      const float* __restrict__ im_w, int ld_w, float* __restrict__ out,
+                                      int* __restrict__ out_counts) {
+  const int b = blockIdx.x, c = blockIdx.y, bc = b * ncls1 + c;
+  const float w = im_w[(size_t)b * ld_w];
+  float* dst = out + (size_t)bc * V * R * 5;
+  int off = 0;
+  for (int v = 0; v < V; ++v) {
+    const int n = max(0, min(tab.counts[v][bc], R));
+    const float* src = tab.dets[v] + (size_t)bc * R * 5;
+    const int fl = tab.flip[v];
+    for (int q = threadIdx.x; q < n * 5; q += blockDim.x) {
+      const int r = q / 5, col = q - r * 5;
+      float x = src[q];
+      if (fl && col == 0) x = flip_x(w, src[r * 5 + 2]);
+      else if (fl && col == 2) x = flip_x(w, src[r * 5]);
+      dst[(size_t)off * 5 + q] = x;
+    }
+    off += n;
+  }
+  if (threadIdx.x == 0) out_counts[bc] = off;
+}
+
+// _get_rois_blob of one keypoint view: (image index, flip_boxes(boxes) * im_scale) — the flip in fp32 as above, the
+// product in fp64 stored fp32.  Without the flip this is scale_rois_kernel with ncols = 4.
+__global__ void aug_scale_rois_kernel(const float* __restrict__ boxes, int ldb, int n, int flip, const float* __restrict__ im_w,
+                                      int ld_w, int per_image, double im_scale, float* __restrict__ rois) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n * 5) return;
+  const int r = i / 5, c = i - r * 5;
+  if (c == 0) { rois[i] = (float)(r / per_image); return; }
+  const float* bx = boxes + (size_t)r * ldb;
+  float x = bx[c - 1];
+  if (flip && (c == 1 || c == 3)) x = flip_x(im_w[(size_t)(r / per_image) * ld_w], bx[c == 1 ? 2 : 0]);
+  rois[i] = (float)((double)x * im_scale);
+}
+}  // namespace dt
+
+extern "C" int dt_aug_merge_dets(const float* const* dets, const int* const* counts, const int* flip, int V, int B,
+                                 int num_classes, int R, const float* im_w, int ld_w, float* out, int* out_counts,
+                                 void* stream) {
+  DT_CHECK_ARG(V >= 1 && V <= DT_AUG_MAX_VIEWS, "dt_aug_merge_dets: V=%d views (1..%d)", V, DT_AUG_MAX_VIEWS);
+  DT_CHECK_ARG(B >= 0 && num_classes >= 2 && R >= 1 && ld_w >= 1, "dt_aug_merge_dets: bad shape B=%d C=%d R=%d ld_w=%d", B,
+               num_classes, R, ld_w);
+  DT_CHECK_ARG((long long)V * R <= DT_NMS_MAX_BOXES, "dt_aug_merge_dets: V*R=%lld exceeds %d", (long long)V * R, DT_NMS_MAX_BOXES);
+  DT_CHECK_ARG(dets && counts && flip, "dt_aug_merge_dets: null view table");
+  if (B == 0) return 0;
+  dt::AugMergeTable tab;
+  memset(&tab, 0, sizeof(tab));
+  for (int v = 0; v < V; ++v) {
+    DT_CHECK_ARG(dets[v] && counts[v], "dt_aug_merge_dets: view %d null pointer", v);
+    tab.dets[v] = dets[v]; tab.counts[v] = counts[v]; tab.flip[v] = flip[v] != 0;
+  }
+  DT_CHECK_ARG(im_w && out && out_counts, "dt_aug_merge_dets: null pointer");
+  dim3 grid(B, num_classes - 1);
+  dt::aug_merge_dets_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(tab, V, num_classes - 1, R, im_w, ld_w, out, out_counts);
+  DT_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int dt_aug_scale_rois(const float* boxes, int ldb, int n, int flip, const float* im_w, int ld_w, int per_image,
+                                 double im_scale, float* rois, void* stream) {
+  DT_CHECK_ARG(n >= 0 && ldb >= 4 && per_image >= 1 && ld_w >= 1, "dt_aug_scale_rois: bad shape n=%d ldb=%d per_image=%d",
+               n, ldb, per_image);
+  if (n == 0) return 0;
+  DT_CHECK_ARG(boxes && rois && (im_w || !flip), "dt_aug_scale_rois: null pointer");
+  dt::aug_scale_rois_kernel<<<(n * 5 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(boxes, ldb, n, flip != 0, im_w, ld_w,
+                                                                                   per_image, im_scale, rois);
+  DT_CHECK_LAUNCH();
+  return 0;
+}

@@ -353,6 +353,11 @@ class DetectionEngine(object):
                                    round_tf32=(self.dtype == cv.TF32), x3_mode=(2 if planar else 1) if self.x3 else 0)
 
     def box_head(self, feats2d, rois, roi_counts, im_info, im_hw):
+        dets, cnt = self.box_head_decode(feats2d, rois, roi_counts, im_info, im_hw)
+        return self.box_nms_limit(dets, cnt)
+
+    def box_head_decode(self, feats2d, rois, roi_counts, im_info, im_hw):
+        """Box head up to box_decode: per class the rows over SCORE_THRESH, dets [B, C-1, R, 5] + counts [B*(C-1)]."""
         torch, cfg, s = self.torch, self.cfg, self.spec
         B, R, _ = rois.shape
         C = s.num_classes
@@ -363,9 +368,14 @@ class DetectionEngine(object):
         o = torch.empty((1, 1, 1, B * R, self.cls_bbox_ld), dtype=torch.float32, device='cuda')
         self.cls_bbox(x, out_f32=True, out=o)
         o2 = o.view(B * R, self.cls_bbox_ld)
-        dets, cnt = rpn_ops.box_decode(rois, roi_counts, o2[:, :C], o2[:, C:5 * C], C, im_info, im_hw,
-                                       cfg.MODEL.BBOX_REG_WEIGHTS, cfg.TEST.SCORE_THRESH, 1)
-        keep, nkeep = box_ops.nms_batched(dets.view(B * (C - 1), R, 5), cnt, cfg.TEST.NMS, box_ops.NMS_2D_GE,
+        return rpn_ops.box_decode(rois, roi_counts, o2[:, :C], o2[:, C:5 * C], C, im_info, im_hw,
+                                  cfg.MODEL.BBOX_REG_WEIGHTS, cfg.TEST.SCORE_THRESH, 1)
+
+    def box_nms_limit(self, dets, cnt):
+        """Per-class NMS and the DETECTIONS_PER_IM limit of dets [B, C-1, R, 5] (R: proposals, or a view union's rows)."""
+        cfg = self.cfg
+        B, C1, R, _ = dets.shape
+        keep, nkeep = box_ops.nms_batched(dets.view(B * C1, R, 5), cnt, cfg.TEST.NMS, box_ops.NMS_2D_GE,
                                           box_ops.ORDER_INDEX)
         return rpn_ops.limit_detections(dets, keep, nkeep, cfg.TEST.DETECTIONS_PER_IM, cap=min(R, self.det_cap))
 
@@ -373,11 +383,20 @@ class DetectionEngine(object):
         """boxes [D, >= 4*Th] image space (fp32 cuda, any row stride), batch_idx [D] fp32 (or None: image index =
         row // per_image) -> xy_preds [D, 4, Th*K].
         2-D heads: feats = per-level centre-frame maps; tube heads: feats = [conv feature 5-D]."""
-        torch, cfg, s = self.torch, self.cfg, self.spec
-        D = boxes.shape[0]
-        Th = s.T_head
+        cfg, s = self.cfg, self.spec
         # _get_rois_blob (test.py:76-113): float64 product, stored fp32, image index in col 0
-        rois = dense_ops.scale_rois(boxes, 4 * Th, im_scale, batch_idx, per_image)
+        rois = dense_ops.scale_rois(boxes, 4 * s.T_head, im_scale, batch_idx, per_image)
+        low = self.keypoint_lowres(feats, rois)
+        D, Th, S = low.shape[:3]
+        return dense_ops.keypoint_decode(low.view(D * Th, S, S, low.shape[4]), boxes, s.K, Th,
+                                         min_size=cfg.KRCNN.INFERENCE_MIN_SIZE, want_heatmaps=want_heatmaps)
+
+    def keypoint_lowres(self, feats, rois, out=None):
+        """Keypoint head up to kps_score_lowres: rois [D, 4*Th+1] (image index, blob-space boxes) -> low-res maps
+        [D, Th, S, S, ld] fp32 (sub-pixel packed; into `out` when given)."""
+        torch, cfg, s = self.torch, self.cfg, self.spec
+        D = rois.shape[0]
+        Th = s.T_head
         res, samp = cfg.KRCNN.ROI_XFORM_RESOLUTION, cfg.KRCNN.ROI_XFORM_SAMPLING_RATIO
         if s.head3d:
             x = self._roi_feats_tube(feats[0], rois, res, samp)               # [D, Th, S, S, C]
@@ -388,10 +407,9 @@ class DetectionEngine(object):
             x = c(x)
         S = x.shape[2]
         ld = (4 * s.K + 3) // 4 * 4
-        low = torch.empty((D, Th, S, S, ld), dtype=torch.float32, device='cuda')
+        low = out if out is not None else torch.empty((D, Th, S, S, ld), dtype=torch.float32, device='cuda')
         self.kps_lowres(x, out_f32=True, out=low)                             # per-frame (kT = 1): time in batch
-        return dense_ops.keypoint_decode(low.view(D * Th, S, S, ld), boxes, s.K, Th,
-                                         min_size=cfg.KRCNN.INFERENCE_MIN_SIZE, want_heatmaps=want_heatmaps)
+        return low
 
     # ------------------------------------------------------------------ tube (3-D) heads
     def _roi_feats_tube(self, feat5d, rois, resolution, sampling):
@@ -517,12 +535,15 @@ class DetectionEngine(object):
         d = self.cfg.TEST.DETECTIONS_PER_IM
         return (d + 4 + 7) // 8 * 8 if d > 0 else self.cfg.TEST.RPN_POST_NMS_TOP_N
 
-    def detect_static(self, frames_u8, want_heatmaps=False):
+    def detect_static(self, frames_u8, want_heatmaps=False, plan=None):
         """The whole path with NO host synchronisation (CUDA-graph capturable): fixed-capacity outputs
-        plus device-side counts.  dets [B, C-1, cap, 5], det_counts [B*(C-1)], xy [B*cap, 4, K]."""
+        plus device-side counts.  dets [B, C-1, cap, 5], det_counts [B*(C-1)], xy [B*cap, 4, K].
+        plan: a core/tta.view_plan of this geometry (TEST.COMPETITION_MODE), or None."""
         torch, s = self.torch, self.spec
         B, T, H, W, _ = frames_u8.shape
         g = self._geom_tensors(B, H, W)
+        if plan is not None:
+            return self._detect_aug(frames_u8, g, plan, want_heatmaps)
         x = self._blob(frames_u8, g['scale'], g['hr'], g['wr'], g['hp'], g['wp'])
         if s.fpn:
             feats = self.link(self.fpn(self.body(x)))
@@ -540,6 +561,60 @@ class DetectionEngine(object):
             else:
                 boxes = dets[:, 0].reshape(B * cap, dets.shape[3])
             out['xy'], out['heat'] = self.keypoint_head(feats, boxes, None, g['scale'], want_heatmaps, per_image=cap)
+        return out
+
+    def _view_features(self, frames_u8, v):
+        """Blob of one test-time view (the clips resized by v.im_scale, mirrored where v.flip) -> centre-frame FPN maps."""
+        B = frames_u8.shape[0]
+        (hr, wr), (hp, wp) = v.size, v.padded
+        x = self._blob_batch([frames_u8[b] for b in range(B)], [v.im_scale] * B, [(hr, wr)] * B, [v.flip] * B, hp, wp)
+        return self.link(self.fpn(self.body(x)))
+
+    def _view_info(self, B, v):
+        key = (B, 'view', v)
+        t = self._geom.get(key)
+        if t is None:
+            t = self._geom[key] = self.torch.tensor([[v.padded[0], v.padded[1], v.im_scale]] * B, dtype=self.torch.float32,
+                                                    device='cuda')
+        return t
+
+    def _detect_aug(self, frames_u8, g, plan, want_heatmaps):
+        """detect_static with test-time augmentation (lib/core/test.py:897-958 in COMPETITION_MODE), FPN graphs with 2-D
+        heads.  Box stage: per view body .. box_decode (only one view's activations live at a time), the union of the
+        views flipped back (UNION / UNION), then per-class NMS and DETECTIONS_PER_IM on it.  Keypoint stage: per view the
+        features again and the head's low-res maps on the view's RoIs; the maps are flipped back, combined (HM_AVG /
+        HM_MAX) and decoded against the final boxes."""
+        torch, cfg, s = self.torch, self.cfg, self.spec
+        if not s.fpn or s.head3d:
+            raise NotImplementedError('test-time augmentation: FPN graphs with 2-D heads only (not tube heads)')
+        B = frames_u8.shape[0]
+        im_hw = g['im_hw']
+        dets_v, cnt_v = [], []
+        for v in plan.box:
+            info = self._view_info(B, v)
+            feats = self._view_features(frames_u8, v)
+            rois, _, roi_counts = self.rpn(feats, info)
+            d, c = self.box_head_decode(feats, rois, roi_counts, info, im_hw)
+            dets_v.append(d)
+            cnt_v.append(c)
+            feats = rois = None                     # release this view's activations before the next view's body
+        union, ucnt = rpn_ops.aug_merge_dets(dets_v, cnt_v, [v.flip for v in plan.box], im_hw)
+        dets_v = cnt_v = None
+        dets, det_counts = self.box_nms_limit(union, ucnt)
+        out = dict(dets=dets, det_counts=det_counts, xy=None, heat=None)
+        if self.kps_convs:
+            cap = dets.shape[2]
+            boxes = dets.view(B * cap, 5) if dets.shape[1] == 1 else dets[:, 0].reshape(B * cap, 5)
+            D, S = B * cap, cfg.KRCNN.ROI_XFORM_RESOLUTION
+            low = torch.empty((len(plan.kps), D, 1, S, S, (4 * s.K + 3) // 4 * 4), dtype=torch.float32, device='cuda')
+            for i, v in enumerate(plan.kps):
+                feats = self._view_features(frames_u8, v)
+                rois = dense_ops.aug_scale_rois(boxes, v.im_scale, v.flip, im_hw, per_image=cap)
+                self.keypoint_lowres(feats, rois, out=low[i])
+                feats = rois = None
+            out['xy'], out['heat'] = dense_ops.keypoint_decode_aug(
+                low.view((len(plan.kps), D, S, S, low.shape[-1])), [v.flip for v in plan.kps], plan.perm, plan.hm_max, boxes,
+                s.K, min_size=cfg.KRCNN.INFERENCE_MIN_SIZE, want_heatmaps=want_heatmaps)
         return out
 
     def gather(self, out):
@@ -563,21 +638,21 @@ class DetectionEngine(object):
         return self.gather(self.detect_static(frames_u8, want_heatmaps))
 
     # ------------------------------------------------------------------ CUDA graph
-    def capture(self, B, T, H, W):
-        """Capture detect_static for a fixed batch geometry.  Returns (static_input, run) where run()
-        replays the graph and returns the static output dict."""
+    def capture(self, B, T, H, W, plan=None):
+        """Capture detect_static (with the test-time augmentation `plan`, or None) for a fixed batch geometry.
+        Returns (static_input, run) where run() replays the graph and returns the static output dict."""
         torch = self.torch
         static_in = torch.zeros((B, T, H, W, 3), dtype=torch.uint8, device='cuda')
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(2):                                     # warm-up: lazy attribute / workspace setup
-                self.detect_static(static_in)
+                self.detect_static(static_in, plan=plan)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            static_out = self.detect_static(static_in)
+            static_out = self.detect_static(static_in, plan=plan)
 
         def run():
             graph.replay()

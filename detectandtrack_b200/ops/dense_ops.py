@@ -150,3 +150,35 @@ def fold_tube_heads(o, R, T, C):
     L.call('dt_fold_tube_heads', L.ptr(o), o.stride(0), R, T, C, L.ptr(cls), L.ptr(bbox),
            L.stream_ptr())
     return cls, bbox
+
+
+def aug_scale_rois(boxes, im_scale, flip=False, im_hw=None, per_image=1):
+    """A test-time view's keypoint RoIs (lib/core/test.py:630-684): boxes [n, >=4] fp32 (row stride free) ->
+    rois [n, 5] = (i // per_image, flip_boxes(boxes) * im_scale), the flip with the width im_hw[i // per_image, 1].
+    Without the flip this is scale_rois(boxes, 4, im_scale, per_image=per_image)."""
+    torch = L.require_cuda()
+    n = boxes.shape[0]
+    assert boxes.dtype == torch.float32 and boxes.stride(1) == 1 and boxes.shape[1] >= 4
+    assert not flip or (im_hw is not None and im_hw.dtype == torch.float32 and im_hw.shape[1] == 2 and im_hw.is_contiguous())
+    rois = torch.empty((n, 5), dtype=torch.float32, device='cuda')
+    w = C.c_void_p(im_hw.data_ptr() + 4) if flip else None
+    L.call('dt_aug_scale_rois', C.c_void_p(boxes.data_ptr()), boxes.stride(0), n, int(bool(flip)), w, 2, int(per_image),
+           float(im_scale), L.ptr(rois), L.stream_ptr())
+    return rois
+
+
+def keypoint_decode_aug(lowres, flips, perm, hm_max, boxes, K=17, min_size=0, want_heatmaps=False):
+    """keypoint_decode of V test-time views combined (lib/core/test.py:686-747), 2-D heads: lowres [V, D, S, S, >=4K]
+    fp32, flips [V], perm [K] (flip_heatmaps' joint swap), hm_max (HM_MAX, else HM_AVG).
+    Returns (xy_preds [D, 4, K], combined heatmaps [D, K, 4S, 4S] or None)."""
+    torch = L.require_cuda()
+    V, D, S, _, ldl = lowres.shape
+    assert V == len(flips) and len(perm) == K
+    assert lowres.dtype == torch.float32 and lowres.is_contiguous()
+    assert boxes.stride(1) == 1 and boxes.dtype == torch.float32
+    xy = L.zeros((D, 4, K), torch.float32)
+    heat = L.zeros((D, K, 4 * S, 4 * S), torch.float32) if want_heatmaps else None
+    L.call('dt_keypoint_decode_aug', L.ptr(lowres), D * S * S * ldl, ldl, S, K, V, (C.c_int * V)(*[int(bool(f)) for f in flips]),
+           (C.c_int * K)(*[int(p) for p in perm]), int(bool(hm_max)), C.c_void_p(boxes.data_ptr()), boxes.stride(0), None, D,
+           int(min_size), L.ptr(heat), L.ptr(xy), L.stream_ptr())
+    return xy, heat

@@ -144,3 +144,21 @@ def generate_proposals_level(logits, deltas, anchors, feat_stride, im_info, pre_
     order = box_ops.ORDER_INDEX if T == 1 else box_ops.ORDER_SCORE
     keep, nkeep = box_ops.nms_batched(props, counts, nms_thresh, cmp_mode, order, max_keep=post_nms_topn)
     return props, keep, nkeep
+
+
+def aug_merge_dets(dets, counts, flips, im_hw):
+    """Test-time augmentation union (lib/core/test.py:338-414, UNION heuristics): V views' box_decode outputs
+    (dets [B, C-1, R, 5], counts [B*(C-1)]) stacked per (image, class) in view order, a view with flips[v] flipped back
+    with the image width im_hw[b, 1].  Returns (union [B, C-1, V*R, 5], counts [B*(C-1)]), nms_batched's layout."""
+    torch = L.require_cuda()
+    V = len(dets)
+    assert V == len(counts) == len(flips) and V >= 1
+    B, C1, R, ld = dets[0].shape
+    assert ld == 5 and all(d.shape == dets[0].shape and d.dtype == torch.float32 and d.is_contiguous() for d in dets)
+    assert im_hw.dtype == torch.float32 and im_hw.shape == (B, 2) and im_hw.is_contiguous()
+    out = L.zeros((B, C1, V * R, 5), torch.float32)
+    cnt = L.zeros((B * C1,), torch.int32)
+    L.call('dt_aug_merge_dets', (C.c_void_p * V)(*[d.data_ptr() for d in dets]),
+           (C.c_void_p * V)(*[c.data_ptr() for c in counts]), (C.c_int * V)(*[int(bool(f)) for f in flips]), V, B, C1 + 1, R,
+           C.c_void_p(im_hw.data_ptr() + 4), 2, L.ptr(out), L.ptr(cnt), L.stream_ptr())
+    return out, cnt

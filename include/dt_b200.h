@@ -269,6 +269,24 @@ int dt_scale_rois(const float* boxes, int ldb, int n, int ncols, const float* bi
 int dt_limit_detections(const float* dets, const int* keep, const int* nkeep, int B, int num_classes, int R,
                         int T, int max_per_im, float* out, int* out_counts, int cap, void* stream);
 
+/* Test-time augmentation (lib/core/test.py:255-414, 630-747), 2-D boxes.  A flip maps x to the original image by
+ * flip_boxes (lib/utils/boxes.py:275-282): x1' = (W - x2) - 1, x2' = (W - x1) - 1 in fp32 with two roundings. */
+#define DT_AUG_MAX_VIEWS 16
+#define DT_KD_AUG_MAX_K 64
+
+/* Union of V views' compacted per-class detections (dt_box_decode's dets [B, C-1, R, 5] and counts [B*(C-1)], device
+ * pointers in the host arrays dets / counts), in view order, each view with flip[v] != 0 flipped back with the image
+ * width im_w[b * ld_w] (device).  out [B, C-1, V*R, 5], out_counts [B*(C-1)]: the layout dt_nms_batched takes.
+ * V*R <= DT_NMS_MAX_BOXES.  No host synchronisation. */
+int dt_aug_merge_dets(const float* const* dets, const int* const* counts, const int* flip, int V, int B, int num_classes,
+                      int R, const float* im_w, int ld_w, float* out, int* out_counts, void* stream);
+
+/* A keypoint view's RoIs: rois [n, 5] = (i / per_image, box' * im_scale), box' = boxes[i, :4] flipped (flip != 0, width
+ * im_w[(i / per_image) * ld_w]) or as is; the product in fp64, stored fp32.  With flip 0 this equals dt_scale_rois
+ * (ncols 4, bidx NULL) byte for byte; im_w may then be NULL. */
+int dt_aug_scale_rois(const float* boxes, int ldb, int n, int flip, const float* im_w, int ld_w, int per_image,
+                      double im_scale, float* rois, void* stream);
+
 /* ---- dense_ops.cu -------------------------------------------------------- */
 
 /* lib/utils/blob.py:40-90 + lib/core/test.py:43-74.  frames [F, H, W, 3] u8 BGR ->
@@ -319,6 +337,15 @@ int dt_roi_align(const void* const* feats, const int* Hs, const int* Ws, const f
 int dt_keypoint_decode(const float* lowres, int ldl, int S, int K, int T, const float* boxes, int ldb,
                        const int* n_dev, int D, int min_size, float* heatmaps, float* xy_preds,
                        void* stream);
+
+/* dt_keypoint_decode of V test-time views combined (lib/core/test.py:686-747), 2-D heads (T = 1).  View v's low-res maps
+ * are lowres + v * view_stride ([D, S, S, ldl] as above); every view's 4S x 4S map is built as dt_keypoint_decode does,
+ * a view with flip[v] != 0 through flip_heatmaps (lib/utils/keypoints.py:81-91: joint perm[k], x mirrored).  hm_max 0
+ * (HM_AVG): fp32 sum in view order, then / V; 1 (HM_MAX): the maximum.  The combined map is decoded against boxes;
+ * heatmaps (may be NULL) [D, K, 4S, 4S] receives it.  flip [V] and perm [K] are host arrays; V <= DT_AUG_MAX_VIEWS. */
+int dt_keypoint_decode_aug(const float* lowres, long long view_stride, int ldl, int S, int K, int V, const int* flip,
+                           const int* perm, int hm_max, const float* boxes, int ldb, const int* n_dev, int D, int min_size,
+                           float* heatmaps, float* xy_preds, void* stream);
 
 /* split-storage modes' conv1: exact fp32 7x7/2 conv + AffineChannel + ReLU on the raw fp32 blob [F, Hp, Wp, Cp];
  * w [7][7][3][64] fp32; y [F, Hp/2, Wp/2, 128] = [hi(64) | lo(64)]: fp32 tf32 pairs (out_bf16 = 0) or bf16
