@@ -14,6 +14,7 @@ import pytest
 
 from test_train_plan import (D_REDUCED, D_ROWS, ROWS, W_REDUCED, W_ROWS, W_FIELDS, dgrad_ref, out_hw, row_dplan, row_wplan,
                              split_ranges, wgrad_key, dgrad_key, wgrad_ref)
+from test_train_reference import rpn_loss_ref as _rpn_loss_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -192,22 +193,6 @@ def test_dgrad_of_every_step_layer_is_bf16_of_the_exact_sum(r):
 
 
 # ---------------------------------------------------------------------------------------------------- dt_rpn_loss_grad
-def _rpn_loss_ref(out, labels, tgt, iw, ow, A, s_cls, s_box, beta):
-    import torch
-    out = out.double()
-    x = out[:, :A]
-    t = labels.double()
-    valid = labels >= 0
-    lc = s_cls * (torch.clamp(x, min=0) - x * t + torch.log1p(torch.exp(-x.abs())))
-    gc = s_cls * (torch.sigmoid(x) - t)
-    d = iw.double() * (out[:, A:5 * A] - tgt.double())
-    ad = d.abs()
-    lb = s_box * ow.double() * torch.where(ad < beta, 0.5 * d * d / beta, ad - 0.5 * beta)
-    gb = s_box * ow.double() * iw.double() * torch.where(ad < beta, d / beta, torch.sign(d))
-    return (torch.where(valid, gc, torch.zeros_like(gc)), gb, float(torch.where(valid, lc, torch.zeros_like(lc)).sum()),
-            float(lb.sum()))
-
-
 def test_rpn_loss_grad_vs_fp64_formulas():
     """SigmoidCrossEntropy + SmoothL1 (beta 1/9) gradients against the fp64 formulas, within the bf16 output bound; ignored
     anchors and the padding channels [5A, ld_g) exactly zero; |d| on both sides of beta; a row count that is not a multiple
