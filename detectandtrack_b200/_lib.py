@@ -79,7 +79,11 @@ HOST_FUNCS = {'dt_planes_ld': ([_i, _i, _i, _i], C.c_int), 'dt_jpeg_available': 
               'dt_aug_merge_dets': ([C.POINTER(_p), C.POINTER(_p), C.POINTER(_i), _i, _i, _i, _i, _p, _i, _p, _p, _p], C.c_int),
               'dt_aug_scale_rois': ([_p, _i, _i, _i, _p, _i, _i, C.c_double, _p, _p], C.c_int),
               'dt_keypoint_decode_aug': ([_p, C.c_longlong, _i, _i, _i, _i, C.POINTER(_i), C.POINTER(_i), _i, _p, _i, _p, _i, _i,
-                                          _p, _p, _p], C.c_int)}
+                                          _p, _p, _p], C.c_int),
+              # TEST.SOFT_NMS / TEST.BBOX_VOTE kernels: launchers too, with their argument-error cases in tests/test_soft_nms.py
+              'dt_soft_nms_batched': ([_p, _i, _i, _i, _p, _f, _f, _f, _i, _p, _p, _p, _p], C.c_int),
+              'dt_box_vote': ([_p, _p, _p, _i, _i, _p, _p, _i, _i, _i, _f, _p, _p, _p], C.c_int)}
+SOFT_NMS_METHODS = {'hard': 0, 'linear': 1, 'gaussian': 2}     # DT_SOFT_NMS_* of include/dt_b200.h
 AUG_MAX_VIEWS = 16                  # DT_AUG_MAX_VIEWS of include/dt_b200.h
 PREP_MAX_CLIPS = 16                 # DT_PREP_MAX_CLIPS of include/dt_b200.h
 

@@ -1,8 +1,9 @@
-"""Drop-in for lib/core/nms_wrapper.py: ``nms(dets, thresh)`` / ``tube_nms``.
+"""Drop-in for lib/core/nms_wrapper.py: ``nms(dets, thresh)`` / ``tube_nms`` / ``soft_nms``.
 Same dispatch (5 columns -> 2-D '>=' NMS returning ascending indices; more ->
 tube NMS returning a score-ordered list), computed by csrc/boxes.cu."""
 import numpy as np
 
+from .. import _lib as L
 from ..ops import box_ops
 
 
@@ -12,6 +13,22 @@ def _run(dets, thresh, cmp_mode, out_order):
     keep, num = box_ops.nms_batched(d, None, thresh, cmp_mode, out_order)
     n = int(num[0].item())
     return keep[0, :n].cpu().numpy().astype(np.int64)
+
+
+def soft_nms(dets, sigma=0.5, overlap_thresh=0.3, score_thresh=0.001, method='linear'):
+    """lib/core/nms_wrapper.py:29-46: (rows [n, 5] fp32, inds [n] int64) as cython_nms.soft_nms returns them, or
+    `dets` itself when it is empty."""
+    if dets.shape[0] == 0:
+        return dets
+    if dets.shape[1] > 5:
+        raise NotImplementedError('Need to handle tubes..')
+    assert method in L.SOFT_NMS_METHODS, 'Unknown soft_nms method: {}'.format(method)
+    import torch
+    d = torch.from_numpy(np.ascontiguousarray(dets, dtype=np.float32)).cuda().unsqueeze(0)
+    rows, inds, num = box_ops.soft_nms_batched(d, None, np.float32(sigma), np.float32(overlap_thresh),
+                                               np.float32(score_thresh), method)
+    n = int(num[0].item())
+    return rows[0, :n].cpu().numpy(), inds[0, :n].cpu().numpy().astype(np.int64)
 
 
 def nms(dets, thresh, soft_nms=False):

@@ -8,7 +8,7 @@ TEST.SCALES = (s,) and TEST.MAX_SIZE = that stage's MAX_SIZE; the identity and H
 TEST.MAX_SIZE.  Every check of what the device path can run lives here (view_plan), before anything is built."""
 import collections
 
-from ..modeling.engine import im_scale_and_size, padded_blob_size
+from ..modeling.engine import check_box_post, im_scale_and_size, padded_blob_size
 
 View = collections.namedtuple('View', 'flip im_scale size padded')
 Plan = collections.namedtuple('Plan', 'box kps hm_max perm')
@@ -47,6 +47,7 @@ def _check(cfg, spec):
                                   'to uint8 before the blob resize) is not on the hot path')
     if spec is not None and (not spec.fpn or spec.head3d):
         raise NotImplementedError('test-time augmentation: FPN graphs with 2-D heads only (not tube heads)')
+    check_box_post(cfg, spec)
 
 
 def _stage(cfg, aug, identity_first, H, W, stride):

@@ -46,6 +46,19 @@ def padded_blob_size(sizes, stride):
     return int(np.ceil(hr / float(stride)) * stride), int(np.ceil(wr / float(stride)) * stride)
 
 
+def check_box_post(cfg, spec):
+    """TEST.SOFT_NMS / TEST.BBOX_VOTE as the device box stage runs them (spec None: skip the graph check).  Raises
+    before anything is built: an unknown SOFT_NMS.METHOD (the reference asserts it, nms_wrapper.py:37-38), and either
+    option with tube heads (the reference's soft_nms raises for tubes, nms_wrapper.py:34-35, and its box_voting would
+    read frame 2's x1 as the score)."""
+    soft, vote = cfg.TEST.SOFT_NMS, cfg.TEST.BBOX_VOTE
+    if soft.ENABLED and soft.METHOD not in L.SOFT_NMS_METHODS:
+        raise ValueError('Unknown soft_nms method: {}'.format(soft.METHOD))
+    if spec is not None and spec.T_head > 1 and (soft.ENABLED or vote.ENABLED):
+        raise NotImplementedError('TEST.SOFT_NMS / TEST.BBOX_VOTE with tube heads (T = %d): the reference handles 2-D '
+                                  'boxes only' % spec.T_head)
+
+
 class _Conv(object):
     """One packed convolution (+ fused epilogue parameters) resident on the device."""
 
@@ -72,11 +85,13 @@ class _Conv(object):
 
 class DetectionEngine(object):
     def __init__(self, cfg, blobs, spec=None, dtype='bf16'):
+        spec = spec or P.GraphSpec(cfg)
+        check_box_post(cfg, spec)                   # before any device work
         torch = L.require_cuda()
         L.lib()
         self.torch = torch
         self.cfg = cfg
-        self.spec = spec or P.GraphSpec(cfg)
+        self.spec = spec
         s = self.spec
         if s.fpn and s.head3d:
             raise NotImplementedError('3-D FPN heads are unimplemented in the reference too (FPN3D.py:228)')
@@ -372,12 +387,39 @@ class DetectionEngine(object):
                                   cfg.MODEL.BBOX_REG_WEIGHTS, cfg.TEST.SCORE_THRESH, 1)
 
     def box_nms_limit(self, dets, cnt):
-        """Per-class NMS and the DETECTIONS_PER_IM limit of dets [B, C-1, R, 5] (R: proposals, or a view union's rows)."""
+        """The per-class post-processing of box_results_with_nms_and_limit (lib/core/test.py:750-806) on the decoded
+        rows dets [B, C-1, R, 4T+1] (R: proposals, or a view union's rows) with counts [B*(C-1)]: hard NMS or
+        TEST.SOFT_NMS, then TEST.BBOX_VOTE against the pre-NMS rows if enabled, then the DETECTIONS_PER_IM limit."""
         cfg = self.cfg
-        B, C1, R, _ = dets.shape
-        keep, nkeep = box_ops.nms_batched(dets.view(B * C1, R, 5), cnt, cfg.TEST.NMS, box_ops.NMS_2D_GE,
-                                          box_ops.ORDER_INDEX)
-        return rpn_ops.limit_detections(dets, keep, nkeep, cfg.TEST.DETECTIONS_PER_IM, cap=min(R, self.det_cap))
+        B, C1, R, ld = dets.shape
+        T = (ld - 1) // 4
+        flat = dets.view(B * C1, R, ld)
+        cap = min(R, self.det_cap)
+        soft, vote = cfg.TEST.SOFT_NMS.ENABLED, cfg.TEST.BBOX_VOTE.ENABLED
+        if not soft:
+            keep, nkeep = box_ops.nms_batched(flat, cnt, cfg.TEST.NMS, box_ops.NMS_TUBE_GT if T > 1 else box_ops.NMS_2D_GE,
+                                              box_ops.ORDER_SCORE if T > 1 else box_ops.ORDER_INDEX)
+            if not vote:
+                return rpn_ops.limit_detections(dets, keep, nkeep, cfg.TEST.DETECTIONS_PER_IM, cap=cap)
+            rows, nrows = box_ops.box_vote(flat, cnt, cfg.TEST.BBOX_VOTE.VOTE_TH, keep=keep, nkeep=nkeep)
+        else:
+            # score_thresh 0.0001 as test.py:777-782 passes it; the reference stores soft_nms's (dets, inds) tuple
+            # there, Detectron unpacks the rows (DESIGN.md §4)
+            rows, _, nrows = box_ops.soft_nms_batched(flat, cnt, cfg.TEST.SOFT_NMS.SIGMA, cfg.TEST.NMS, 0.0001,
+                                                      cfg.TEST.SOFT_NMS.METHOD)
+            if vote:
+                rows, nrows = box_ops.box_vote(flat, cnt, cfg.TEST.BBOX_VOTE.VOTE_TH, top=rows, top_counts=nrows)
+        return rpn_ops.limit_detections(rows.view(B, C1, R, 5), self._identity_keep(B * C1, R), nrows,
+                                        cfg.TEST.DETECTIONS_PER_IM, cap=cap)
+
+    def _identity_keep(self, n, R):
+        """keep [n, R] = 0..R-1 per list: dt_limit_detections over rows that are already the survivors (built once per
+        geometry, outside any capture)."""
+        key = ('identity_keep', n, R)
+        t = self._geom.get(key)
+        if t is None:
+            t = self._geom[key] = self.torch.from_numpy(np.tile(np.arange(R, dtype=np.int32), (n, 1))).cuda()
+        return t
 
     def keypoint_head(self, feats, boxes, batch_idx, im_scale, want_heatmaps=False, per_image=1):
         """boxes [D, >= 4*Th] image space (fp32 cuda, any row stride), batch_idx [D] fp32 (or None: image index =
@@ -455,10 +497,7 @@ class DetectionEngine(object):
         cls, bbox = dense_ops.fold_tube_heads(o.view(n * T, self.cls_bbox_ld), n, T, C)
         dets, cnt = rpn_ops.box_decode(rois, roi_counts, cls, bbox, C, im_info, im_hw, cfg.MODEL.BBOX_REG_WEIGHTS,
                                        cfg.TEST.SCORE_THRESH, T)
-        keep, nkeep = box_ops.nms_batched(dets.view(B * (C - 1), R, 4 * T + 1), cnt, cfg.TEST.NMS,
-                                          box_ops.NMS_TUBE_GT if T > 1 else box_ops.NMS_2D_GE,
-                                          box_ops.ORDER_SCORE if T > 1 else box_ops.ORDER_INDEX)
-        return rpn_ops.limit_detections(dets, keep, nkeep, cfg.TEST.DETECTIONS_PER_IM, cap=min(R, self.det_cap))
+        return self.box_nms_limit(dets, cnt)
 
     # ------------------------------------------------------------------ end to end
     def blob_geometry(self, h, w):

@@ -59,7 +59,44 @@ def nms_batched(dets, counts=None, thresh=0.5, cmp_mode=None, out_order=None, ma
     return keep, num
 
 
-ALGOS = {'hungarian': 0, 'greedy': 1}
+def soft_nms_batched(dets, counts=None, sigma=0.5, overlap_thresh=0.3, score_thresh=0.001, method='linear'):
+    """lib/core/nms_wrapper.py:29-46 soft_nms per list: dets [B, Nmax, >=5] cuda fp32 (2-D boxes + score), counts [B]
+    int32 (or None).  Returns (rows [B, Nmax, 5], inds [B, Nmax] int32 source rows, counts [B] int32)."""
+    torch = L.require_cuda()
+    if method not in L.SOFT_NMS_METHODS:
+        raise ValueError('Unknown soft_nms method: {}'.format(method))
+    dets = _f32c(dets, torch)
+    B, nmax, ld = dets.shape
+    out = torch.empty((B, max(nmax, 1), 5), dtype=torch.float32, device='cuda')
+    inds = torch.empty((B, max(nmax, 1)), dtype=torch.int32, device='cuda')
+    num = L.zeros((B,), torch.int32)
+    if counts is not None:
+        counts = counts.to(device='cuda', dtype=torch.int32).contiguous()
+    L.call('dt_soft_nms_batched', L.ptr(dets), B, nmax, ld, L.ptr(counts), float(sigma), float(overlap_thresh),
+           float(score_thresh), L.SOFT_NMS_METHODS[method], L.ptr(out), L.ptr(inds), L.ptr(num), L.stream_ptr())
+    return out, inds, num
+
+
+def box_vote(all_dets, all_counts, thresh, top=None, top_counts=None, keep=None, nkeep=None):
+    """lib/utils/boxes.py:294-310 box_voting per list: the top rows voted against all_dets [B, Nmax, >=5] (counts
+    all_counts [B] or None).  Top rows: keep [B, Nmax] / nkeep [B] (nms_batched's output, rows of all_dets), or
+    top [B, Ntop, >=5] / top_counts [B] (soft_nms_batched's output).  Returns (rows [B, Ntop, 5], counts [B] int32)."""
+    torch = L.require_cuda()
+    all_dets = _f32c(all_dets, torch)
+    B, nmax, ld = all_dets.shape
+    if keep is not None:
+        keep, top_counts, ntop, ld_top = keep.contiguous(), nkeep, nmax, 0
+    else:
+        top = _f32c(top, torch)
+        ntop, ld_top = top.shape[1], top.shape[2]
+    out = torch.empty((B, max(ntop, 1), 5), dtype=torch.float32, device='cuda')
+    num = L.zeros((B,), torch.int32)
+    L.call('dt_box_vote', L.ptr(top), L.ptr(keep), L.ptr(top_counts.contiguous()), ntop, ld_top, L.ptr(all_dets),
+           L.ptr(all_counts), B, nmax, ld, float(thresh), L.ptr(out), L.ptr(num), L.stream_ptr())
+    return out, num
+
+
+ALGOS ={'hungarian': 0, 'greedy': 1}
 
 
 def lsa_batched(cost, nrows, ncols, algo='hungarian'):

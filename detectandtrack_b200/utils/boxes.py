@@ -25,6 +25,24 @@ def bbox_overlaps(boxes, query_boxes):
     return box_ops.bbox_overlaps(torch.from_numpy(b).cuda(), torch.from_numpy(q).cuda(), T=T).cpu().numpy()
 
 
+def box_voting(top_dets, all_dets, thresh):
+    """lib/utils/boxes.py:294-310: each row of top_dets [N, 5] with its box replaced by the score-weighted average of
+    the all_dets [M, 5] boxes whose IoU with it is >= thresh (computed on the device)."""
+    import torch
+    top = np.asarray(top_dets)
+    if top.shape[1] != 5 or np.asarray(all_dets).shape[1] != 5:
+        raise NotImplementedError('box_voting: 2-D boxes [N, 5] only, got %s / %s' % (top.shape, np.asarray(all_dets).shape))
+    out = top.copy()
+    if top.shape[0] == 0:
+        return out
+    a = torch.from_numpy(np.ascontiguousarray(all_dets, dtype=np.float32)).cuda().unsqueeze(0)
+    t = torch.from_numpy(np.ascontiguousarray(top, dtype=np.float32)).cuda().unsqueeze(0)
+    n = torch.tensor([top.shape[0]], dtype=torch.int32, device='cuda')
+    rows, _ = box_ops.box_vote(a, None, thresh, top=t, top_counts=n)
+    out[:, :4] = rows[0, :top.shape[0], :4].cpu().numpy()
+    return out
+
+
 def boxes_area(boxes):
     """lib/utils/boxes.py:72-78."""
     w = (boxes[:, 2::4] - boxes[:, 0::4] + 1)

@@ -73,6 +73,30 @@ int dt_nms_batched(const float* dets, int batch, int nmax, int ld, int T, const 
                    float thresh, int cmp_mode, int out_order, int max_keep, int* keep,
                    int* num_keep, void* workspace, size_t workspace_bytes, void* stream);
 
+/* TEST.SOFT_NMS.METHOD (lib/core/nms_wrapper.py:37) */
+#define DT_SOFT_NMS_HARD 0
+#define DT_SOFT_NMS_LINEAR 1
+#define DT_SOFT_NMS_GAUSSIAN 2
+
+/* lib/core/nms_wrapper.py:29-46 soft_nms -> lib/utils/cython_nms.pyx:98-203, batched, 2-D boxes.
+ * dets [batch, nmax, ld] (ld >= 5: columns 0..3 box, 4 score), counts [batch] (device) valid rows, NULL = nmax.
+ * out [batch, nmax, 5] receives the surviving rows (original coordinates, decayed scores) in the reference's row
+ * order, out_inds [batch, nmax] (may be NULL) the source row of each, out_counts [batch] their number.
+ * Nt: overlap threshold of the linear / hard methods; threshold: rows whose decayed score falls below it are dropped.
+ * Bit-exact with the compiled reference.  nmax <= DT_NMS_MAX_BOXES.  No host synchronisation. */
+int dt_soft_nms_batched(const float* dets, int batch, int nmax, int ld, const int* counts, float sigma, float Nt,
+                        float threshold, int method, float* out, int* out_inds, int* out_counts, void* stream);
+
+/* lib/utils/boxes.py:294-310 box_voting, batched: each top row's box becomes the score-weighted np.average of the
+ * boxes of `all` [batch, nmax, ld] (counts all_counts, NULL = nmax) whose IoU with it is >= thresh; its score is kept.
+ * Top rows: with top_keep [batch, nmax] (dt_nms_batched's keep), rows top_keep[b, :top_counts[b]] of `all` (top is
+ * then unused and top_nmax must equal nmax); else top [batch, top_nmax, ld_top] rows :top_counts[b] (dt_soft_nms_batched's
+ * output).  out [batch, top_nmax, 5] in the top order, out_counts [batch] = top_counts.  Bit-exact with the reference
+ * under numpy 2.x.  No host synchronisation. */
+int dt_box_vote(const float* top, const int* top_keep, const int* top_counts, int top_nmax, int ld_top,
+                const float* all, const int* all_counts, int batch, int nmax, int ld, float thresh, float* out,
+                int* out_counts, void* stream);
+
 /* ---- lsa.cu ------------------------------------------------------------- */
 
 /* scipy.optimize.linear_sum_assignment as called at
