@@ -82,8 +82,16 @@ HOST_FUNCS = {'dt_planes_ld': ([_i, _i, _i, _i], C.c_int), 'dt_jpeg_available': 
                                           _p, _p, _p], C.c_int),
               # TEST.SOFT_NMS / TEST.BBOX_VOTE kernels: launchers too, with their argument-error cases in tests/test_soft_nms.py
               'dt_soft_nms_batched': ([_p, _i, _i, _i, _p, _f, _f, _f, _i, _p, _p, _p, _p], C.c_int),
-              'dt_box_vote': ([_p, _p, _p, _i, _i, _p, _p, _i, _i, _i, _f, _p, _p, _p], C.c_int)}
+              'dt_box_vote': ([_p, _p, _p, _i, _i, _p, _p, _i, _i, _i, _f, _p, _p, _p], C.c_int),
+              # TRACKING.FLOW_SMOOTHING_ON kernels: launchers too, with their argument-error cases in tests/test_flow.py
+              'dt_bgr_to_gray': ([_p, C.c_longlong, _p, _p], C.c_int),
+              'dt_farneback_workspace_bytes': ([_i, _i, _i, _i, C.POINTER(_sz)], C.c_int),
+              'dt_farneback_flow': ([_p, _i, _i, _i, _p, _i, C.c_double, _i, _i, _i, _i, C.c_double, _i, _p, _p, _sz, _p], C.c_int),
+              'dt_flow_mean_abs': ([_p, _i, _i, _i, _p, _p], C.c_int),
+              'dt_flow_smooth_poses': ([_p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _i, _p, _p, _i, _p, _p, _p], C.c_int)}
 SOFT_NMS_METHODS = {'hard': 0, 'linear': 1, 'gaussian': 2}     # DT_SOFT_NMS_* of include/dt_b200.h
+FARNEBACK_GAUSSIAN = 256           # DT_FARNEBACK_GAUSSIAN of include/dt_b200.h (cv2.OPTFLOW_FARNEBACK_GAUSSIAN)
+FLOW_MAX_CONTEXT = 16              # DT_FLOW_MAX_CONTEXT of include/dt_b200.h
 AUG_MAX_VIEWS = 16                  # DT_AUG_MAX_VIEWS of include/dt_b200.h
 PREP_MAX_CLIPS = 16                 # DT_PREP_MAX_CLIPS of include/dt_b200.h
 

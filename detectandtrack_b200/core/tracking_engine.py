@@ -15,6 +15,12 @@ into one [F, Dmax, 4T+1] tensor and three launches do the work
 Only the 'bbox-overlap' cost runs on the device (the configuration of every shipped yaml; the
 weights of the other costs are 0, config.py:550-551), with 'hungarian' or 'greedy' matching;
 anything else raises NotImplementedError.
+
+TRACKING.FLOW_SMOOTHING_ON (:401-643) runs after the id pass, one video at a time: Farneback flow
+between consecutive key frames (csrc/flow.cu, all pairs of a frame size in one call), the shot-boundary
+test np.abs(flow).mean() > FLOW_SHOT_BOUNDARY_TH on the device, then one launch that shifts every pose
+±N_CONTEXT_FRAMES along the flow and combines the shifts per track.  Only the output track order of each
+frame (the reference's list(set(...)), CPython's set order) is computed on the host.
 """
 import logging
 import os.path as osp
@@ -250,11 +256,152 @@ def _compute_tracks_video(video_json_data, dets):
     return _tracks_for_videos([boxes], [poses])[0]
 
 
+# ------------------------------------------------------------------------------ flow smoothing
+def _check_tracking_options(dets):
+    """Rejects, before any device work, what the device path does not run: LSTM tracking, and flow smoothing with
+    anything but centre-frame boxes (T = 1) and [4, 17] poses (the shapes _weighted_avg_poses and _combine_boxes
+    take, :454-479) or with the FLOW_SMOOTHING_COMBINE debugger hook."""
+    if cfg.TRACKING.LSTM_TEST.LSTM_TRACKING_ON:
+        raise NotImplementedError('LSTM tracking is outside the device path')
+    if not cfg.TRACKING.FLOW_SMOOTHING_ON:
+        return
+    if cfg.TRACKING.DEBUG.FLOW_SMOOTHING_COMBINE:
+        raise NotImplementedError('TRACKING.DEBUG.FLOW_SMOOTHING_COMBINE (a pdb hook) is not on the device path')
+    n = cfg.TRACKING.FLOW_SMOOTHING.N_CONTEXT_FRAMES
+    assert n >= 0                                                   # :612
+    if n > FLOW_MAX_CONTEXT:
+        raise NotImplementedError('N_CONTEXT_FRAMES=%d exceeds %d' % (n, FLOW_MAX_CONTEXT))
+    for i, b in enumerate(dets['all_boxes'][1]):
+        if len(b) and np.shape(b)[-1] != 5:
+            raise NotImplementedError('flow smoothing takes centre-frame boxes (4T+1 = 5 columns); image %d has %d'
+                                      % (i, np.shape(b)[-1]))
+    for i, ps in enumerate(dets['all_keyps'][1]):
+        for p in ps:
+            if np.shape(p) != (4, 17):
+                raise NotImplementedError('flow smoothing takes [4, 17] poses (17 centre-frame joints); image %d has %s'
+                                          % (i, np.shape(p)))
+
+
+FLOW_MAX_CONTEXT = 16        # DT_FLOW_MAX_CONTEXT of include/dt_b200.h
+FLOW_MAX_PAIRS = 32          # pairs per dt_farneback_flow call (bounds the memory: about 90 MB per 720p pair)
+
+
+def read_key_frame(entry):
+    """lib/utils/image.py:65-79 read_image_video(entry, key_frame_only=True): the centre frame of a clip entry
+    (get_image_path, :44-48) as BGR uint8.  Synthetic entries take test_engine's seeded frame of that index."""
+    if entry.get('synthetic'):
+        from .test_engine import _synthetic_frame
+        T = cfg.VIDEO.NUM_FRAMES if cfg.MODEL.VIDEO_ON else 1
+        return _synthetic_frame(entry['height'], entry['width'], entry['seed'], T // 2)
+    import cv2
+    path = _image_path(entry)
+    im = cv2.imread(path)
+    assert im is not None, 'could not read {}'.format(path)
+    return im
+
+
+def _read_key_frames(video_json_data):
+    """read_key_frame of every entry, on loader threads."""
+    from concurrent.futures import ThreadPoolExecutor
+    with ThreadPoolExecutor(max_workers=8) as ex:
+        return list(ex.map(lambda e: np.ascontiguousarray(read_key_frame(e[0]), dtype=np.uint8), video_json_data))
+
+
+def compute_optical_flow(video_json_data):
+    """:573-597.  Returns (flows, means): flows[i] the cuda fp32 [H, W, 2] flow of key frame i -> i + 1 (None for a
+    pair of different frame sizes, where cv2 raises), means[i] = np.abs(flows[i]).mean() as np.float32."""
+    import torch
+    from ..ops import flow_ops
+    frames = _read_key_frames(video_json_data)
+    n = len(frames)
+    flows, means = [None] * max(n - 1, 0), [None] * max(n - 1, 0)
+    i = 0
+    while i < n - 1:
+        j = i                                  # frames i..j share one size; pairs i..j-1 go to the device in chunks
+        while j + 1 < n and frames[j + 1].shape == frames[i].shape:
+            j += 1
+        for a in range(i, j, FLOW_MAX_PAIRS):
+            b = min(a + FLOW_MAX_PAIRS, j)
+            clip = torch.from_numpy(np.stack(frames[a:b + 1])).cuda()
+            f = flow_ops.farneback_flow(clip, [(k, k + 1) for k in range(b - a)])
+            m = flow_ops.flow_mean_abs(f).cpu().numpy()
+            for k in range(b - a):
+                flows[a + k], means[a + k] = f[k], m[k]
+        i = j + 1
+    return flows, means
+
+
+def _output_tracks(tracks, counts, moves, n_context, extend):
+    """The track list of every frame after _combine_shifted_poses (:491-498): shift s of frame f holds the tracks of
+    frame f - s when that frame has detections and the chain of pairs between them moves (``moves[q]``: the pair
+    q -> q + 1 has a flow below the shot-boundary threshold)."""
+    n = len(tracks)
+    out = []
+    for f in range(n):
+        if not extend:
+            out.append(list(tracks[f]))
+            continue
+        ids = set()
+        for s in range(-n_context, n_context + 1):
+            g = f - s
+            if 0 <= g < n and counts[g] and all(moves[q] for q in range(min(g, f), max(g, f))):
+                ids |= set(tracks[g])
+        out.append(list(ids))
+    return out
+
+
+def _smooth_pose_video(video_json_data, dets, tracks):
+    """:600-643.  Replaces the poses and boxes of the video's images with the flow-smoothed ones and returns the
+    new per-frame track lists."""
+    import torch
+    from ..ops import flow_ops
+    ncontext = cfg.TRACKING.FLOW_SMOOTHING.N_CONTEXT_FRAMES
+    assert ncontext >= 0
+    n = len(video_json_data)
+    if n == 0:
+        return []
+    poses = [_get_poses(dets, det_id) for (_, det_id) in video_json_data]
+    boxes = [_get_boxes(dets, det_id) for (_, det_id) in video_json_data]
+    counts = [len(t) for t in tracks]
+    for f in range(n):
+        assert len(poses[f]) == len(boxes[f]) == counts[f], 'frame %d: poses, boxes and tracks differ in number' % f
+    flows, moves = [None] * n, [False] * n
+    if ncontext > 0 and n > 1:
+        fl, means = compute_optical_flow(video_json_data)
+        th = cfg.TRACKING.FLOW_SMOOTHING.FLOW_SHOT_BOUNDARY_TH
+        for q in range(n - 1):
+            flows[q] = fl[q]
+            moves[q] = fl[q] is not None and not (means[q] > th)        # :404-407
+    out_tracks = _output_tracks(tracks, counts, moves, ncontext, cfg.TRACKING.FLOW_SMOOTHING.EXTEND_TRACKS)
+    dmax = max(max(counts), 1)
+    packed_b, _ = _pack(boxes, ld=5)
+    packed_p = _pack_poses(poses, dmax, 17)
+    packed_t = np.full((n, dmax), -1, dtype=np.int32)
+    for f in range(n):
+        packed_t[f, :counts[f]] = tracks[f]
+    ocounts = np.array([len(t) for t in out_tracks], dtype=np.int32)
+    omax = max(int(ocounts.max()), 1)
+    packed_o = np.zeros((n, omax), dtype=np.int32)
+    for f in range(n):
+        packed_o[f, :ocounts[f]] = out_tracks[f]
+    is_start = np.zeros(n, dtype=np.uint8)
+    is_start[0] = 1
+    p, b = flow_ops.smooth_poses(packed_p, packed_b[:, :dmax], counts, packed_t, is_start, flows,
+                                 np.array([not m for m in moves], dtype=np.uint8), ncontext, packed_o, ocounts)
+    p, b = p.cpu().numpy(), b.cpu().numpy()
+    for f, (_, det_id) in enumerate(video_json_data):
+        k = int(ocounts[f])
+        dets['all_keyps'][1][det_id] = [p[f, o].copy() for o in range(k)]
+        # a frame left without tracks gets np.zeros((0, box_size)), fp64 as in the reference (:541-544)
+        dets['all_boxes'][1][det_id] = b[f, :k].copy() if k else np.zeros((0, boxes[f].shape[-1]))
+    return out_tracks
+
+
 def compute_matches_tracks(json_data, dets, lstm_model=None):
     """:669-708.  Splits images into videos by dirname, links every video in one
-    batched device pass, writes dets['all_tracks'] = [[], per-image id lists]."""
-    if cfg.TRACKING.LSTM_TEST.LSTM_TRACKING_ON or cfg.TRACKING.FLOW_SMOOTHING_ON:
-        raise NotImplementedError('LSTM tracking / flow smoothing are outside the device path')
+    batched device pass, writes dets['all_tracks'] = [[], per-image id lists].
+    With TRACKING.FLOW_SMOOTHING_ON each video's poses and boxes are then smoothed along the flow (:695-697)."""
+    _check_tracking_options(dets)
     num_imgs = len(json_data)
     all_tracks = [[]] * num_imgs
     all_video_roidb, video_entries = [], []
@@ -271,6 +418,8 @@ def compute_matches_tracks(json_data, dets, lstm_model=None):
     vids = [[_get_boxes(dets, det_id) for (_, det_id) in v] for v in all_video_roidb]
     vposes = [[_get_poses(dets, det_id) for (_, det_id) in v] for v in all_video_roidb]
     tracks = _tracks_for_videos(vids, vposes)
+    if cfg.TRACKING.FLOW_SMOOTHING_ON:
+        tracks = [_smooth_pose_video(entries, dets, tracks[v]) for v, entries in enumerate(all_video_roidb)]
     for v, entries in enumerate(all_video_roidb):
         for i, (_, det_id) in enumerate(entries):
             all_tracks[det_id] = tracks[v][i]
@@ -293,6 +442,7 @@ def run_posetrack_tracking(test_output_dir, json_data, write_json=True):
         _center_detections(dets)
     assert len(json_data) == len(dets['all_boxes'][1])
     assert len(json_data) == len(dets['all_keyps'][1])
+    _check_tracking_options(dets)
     conf = cfg.TRACKING.CONF_FILTER_INITIAL_DETS
     logger.info('Pruning detections with less than %s confidence', conf)
     dets = _prune_bad_detections(dets, json_data, conf)

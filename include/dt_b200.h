@@ -567,6 +567,34 @@ int dt_sample_rois(const float* rois, const float* roi_scores, const int* roi_co
                    float* inside_weights, float* outside_weights, int* out_counts, float* kp_rois, int* kp_locations,
                    float* kp_weights, int* kp_counts, int kcap, float* totals, void* stream);
 
+/* ---- flow.cu: TRACKING.FLOW_SMOOTHING_ON (lib/core/tracking_engine.py:401-643) --------------------------- */
+
+#define DT_FARNEBACK_GAUSSIAN 256       /* cv2.OPTFLOW_FARNEBACK_GAUSSIAN, the only window implemented */
+#define DT_FLOW_MAX_CONTEXT 16          /* TRACKING.FLOW_SMOOTHING.N_CONTEXT_FRAMES */
+
+/* cvtColor(BGR2GRAY) of npix uint8 BGR pixels in OpenCV 4.x's 15-bit fixed point (bit-exact). */
+int dt_bgr_to_gray(const uint8_t* bgr, long long npix, uint8_t* gray, void* stream);
+/* Workspace of dt_farneback_flow for nframes frames of H x W and npairs pairs. */
+int dt_farneback_workspace_bytes(int H, int W, int nframes, int npairs, size_t* bytes /*host out*/);
+/* cv2.calcOpticalFlowFarneback(gray[a], gray[b], None, pyr_scale, levels, winsize, iterations, poly_n, poly_sigma, flags)
+ * (OpenCV 4.x CPU algorithm) for every pair (a, b) of pairs [npairs, 2] (device int32 frame indices) at once.  frames
+ * [nframes, H, W, 3] uint8 BGR, converted to gray as dt_bgr_to_gray does; flows out [npairs, H, W, 2] fp32.  flags must
+ * be DT_FARNEBACK_GAUSSIAN, poly_n 5 or 7, winsize <= 347. */
+int dt_farneback_flow(const uint8_t* frames, int nframes, int H, int W, const int* pairs, int npairs, double pyr_scale,
+                      int levels, int winsize, int iterations, int poly_n, double poly_sigma, int flags, float* flows,
+                      void* workspace, size_t workspace_bytes, void* stream);
+/* out[p] = np.abs(flows[p]).mean() for flows [npairs, H, W, 2] fp32: numpy's fp32 pairwise sum, bit for bit. */
+int dt_flow_mean_abs(const float* flows, int npairs, int H, int W, float* out, void* stream);
+/* _shift_poses + _combine_shifted_poses (:401-546), bit-exact, for F frames of packed videos: poses [F, dmax, 4, K],
+ * boxes [F, dmax, 5] (T = 1), counts [F], tracks [F, dmax] (dt_assign_track_ids' output), is_start [F] (first frame of a
+ * video).  flows [F] (device array of device pointers): the flow of frame f -> f + 1 as [H, W, 2] fp32 with flow_hw [F, 2]
+ * = (H, W); no_flow [F] marks a pair that moves nothing (no flow, or a shot boundary).  out_tracks [F, omax] / out_counts
+ * [F]: the output track order of each frame (computed on the host); out_poses [F, omax, 4, K], out_boxes [F, omax, 5]. */
+int dt_flow_smooth_poses(const float* poses, const float* boxes, const int* counts, const int* tracks,
+                         const unsigned char* is_start, int F, int dmax, int K, const float* const* flows, const int* flow_hw,
+                         const unsigned char* no_flow, int n_context, const int* out_tracks, const int* out_counts, int omax,
+                         float* out_poses, float* out_boxes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
