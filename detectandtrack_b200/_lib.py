@@ -88,7 +88,13 @@ HOST_FUNCS = {'dt_planes_ld': ([_i, _i, _i, _i], C.c_int), 'dt_jpeg_available': 
               'dt_farneback_workspace_bytes': ([_i, _i, _i, _i, C.POINTER(_sz)], C.c_int),
               'dt_farneback_flow': ([_p, _i, _i, _i, _p, _i, C.c_double, _i, _i, _i, _i, C.c_double, _i, _p, _p, _sz, _p], C.c_int),
               'dt_flow_mean_abs': ([_p, _i, _i, _i, _p, _p], C.c_int),
-              'dt_flow_smooth_poses': ([_p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _i, _p, _p, _i, _p, _p, _p], C.c_int)}
+              'dt_flow_smooth_poses': ([_p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _i, _p, _p, _i, _p, _p, _p], C.c_int),
+              # Winograd keypoint head: launchers too, with their argument-error cases in tests/test_winograd.py
+              'dt_wino_gemm': ([_p, _p, _p, _i, _i, _i, _p], C.c_int),
+              'dt_wino_plan': ([_i, _i, _i, C.c_void_p], C.c_int),
+              'dt_wino_input': ([_p, _i, _i, _i, _p, _p], C.c_int),
+              'dt_wino_output_input': ([_p, _i, _i, _i, _p, _i, _p, _p], C.c_int),
+              'dt_wino_output': ([_p, _i, _i, _i, _p, _i, _p, _p], C.c_int)}
 SOFT_NMS_METHODS = {'hard': 0, 'linear': 1, 'gaussian': 2}     # DT_SOFT_NMS_* of include/dt_b200.h
 FARNEBACK_GAUSSIAN = 256           # DT_FARNEBACK_GAUSSIAN of include/dt_b200.h (cv2.OPTFLOW_FARNEBACK_GAUSSIAN)
 FLOW_MAX_CONTEXT = 16              # DT_FLOW_MAX_CONTEXT of include/dt_b200.h

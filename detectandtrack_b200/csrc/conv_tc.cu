@@ -207,8 +207,10 @@ __device__ __forceinline__ LiveTaps tile_live(const ConvKernelParams& p, const T
 // epilogue's path.  The epilogue is unrolled over a whole tile's 64 (row, 8-column group) pairs per thread, so every
 // runtime branch in it is 64 copies of code; compiled for one path it is a third of the size, and one warpgroup running
 // it alone measured 2.5x slower on the K-light layers when it carried all paths.
+// WTAP: the weight box's tap coordinate is the tile's image index (dt_wino_gemm: image = Winograd component xi, so one
+// pointwise launch runs the 16 products V_xi * U_xi^T); false for every dt_conv3d / dt_conv1_7x7s2 launch.
 constexpr int RES_TMA = 1, RES_LDG = 2;
-template <int BN, int KIND, bool SPLIT, int NMMA, bool OUT_F32, int RES>
+template <int BN, int KIND, bool SPLIT, int NMMA, bool OUT_F32, int RES, bool WTAP = false>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
@@ -339,7 +341,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           for (int q = 0; q < 2; ++q) {
             if (load_b) {
               const int2 e = tabB[jq[q]];
-              x0[q] = e.x; x1[q] = n_base; x2[q] = e.y; x3[q] = 0;
+              x0[q] = e.x; x1[q] = n_base; x2[q] = WTAP ? e.y + n : e.y; x3[q] = 0;
             } else {
               const int4 e = tabA[jq[q]];
               x0[q] = e.x; x1[q] = w_base + e.y; x2[q] = h_base + e.z; x3[q] = t_base + e.w;
@@ -817,12 +819,12 @@ static double conv_mma_kblocks(const dt_conv_desc* d, const ConvGeom& g) {
   return (double)g.nmma * g.kchunks * cdiv(d->Cout, g.BN) * cdiv(d->N, ts.tb) * st * sh * sw;
 }
 
-template <int BN, int KIND, bool SPLIT, int NMMA, bool OUT_F32, int RES>
+template <int BN, int KIND, bool SPLIT, int NMMA, bool OUT_F32, int RES, bool WTAP = false>
 static int launch_conv0(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
                         const ConvKernelParams& p, int grid, cudaStream_t stream) {
   using Cfg = ConvCfg<BN>;
   static DynSmemGrant grant;
-  DT_CHECK_CUDA(grant_dyn_smem(conv_tc_kernel<BN, KIND, SPLIT, NMMA, OUT_F32, RES>, Cfg::BUDGET, &grant));
+  DT_CHECK_CUDA(grant_dyn_smem(conv_tc_kernel<BN, KIND, SPLIT, NMMA, OUT_F32, RES, WTAP>, Cfg::BUDGET, &grant));
   ConvKernelParams q = p;
   const int groups = p.kT * p.kH * p.kW * p.kchunks;
   DT_CHECK_ARG(groups <= 2048, "conv: %d (tap, channel chunk) groups per tile exceed the schedule table", groups);
@@ -841,7 +843,7 @@ static int launch_conv0(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = at; lc.numAttrs = pdl ? 1 : 0;
-  DT_CHECK_CUDA(cudaLaunchKernelEx(&lc, conv_tc_kernel<BN, KIND, SPLIT, NMMA, OUT_F32, RES>, tmA, tmB, tmC, tmR, q));
+  DT_CHECK_CUDA(cudaLaunchKernelEx(&lc, conv_tc_kernel<BN, KIND, SPLIT, NMMA, OUT_F32, RES, WTAP>, tmA, tmB, tmC, tmR, q));
   return 0;
 }
 
@@ -1063,6 +1065,96 @@ extern "C" int dt_conv_plan(const dt_conv_desc* d, int residual_aligned, dt_conv
   }
   o->mma_kblocks = conv_mma_kblocks(d, g);
   return 0;
+}
+
+
+// Winograd F(2x2, 3x3) GEMM of the bf16x3 keypoint head (wino.cu holds the transforms): M_xi = V_xi * U_xi^T for the
+// 16 components xi, as ONE pointwise split-operand launch of the conv kernel.  The map is (C, W = G tiles, 1, 1,
+// N = 16): image n of the launch is component n, and its weight box is tap n of the packed U (WTAP).  The M tile is
+// 128 consecutive Winograd tiles of one component (TB = 1, so no tile straddles two components); the k order of an
+// output element is the Cin / 64 channel chunks in order, whatever G is.
+static int wino_check(const char* fn, int G, int Cin, int Cout) {
+  DT_CHECK_ARG(G >= 1 && Cin >= 64 && Cin % 64 == 0 && Cout >= 128 && Cout % 128 == 0,
+               "%s: bad shape G=%d Cin=%d Cout=%d (Cin %% 64 == 0, Cout %% 128 == 0)", fn, G, Cin, Cout);
+  DT_CHECK_ARG((long long)16 * cdiv(G, 128) * (Cout / 128) < (1ll << 31), "%s: too many tiles (G=%d)", fn, G);
+  return 0;
+}
+
+static dt_conv_desc wino_desc(int G, int Cin, int Cout) {
+  dt_conv_desc d;
+  memset(&d, 0, sizeof(d));
+  d.N = 16; d.Ti = 1; d.Hi = 1; d.Wi = G; d.Cin = Cin; d.Cout = Cout;
+  d.kT = d.kH = d.kW = 1; d.sT = d.sH = d.sW = 1;
+  d.in_ld = 2 * Cin; d.w_ld = 2 * Cin; d.out_ld = Cout;
+  d.dtype = DT_DTYPE_BF16; d.out_f32 = 1; d.x3 = 1;
+  return d;
+}
+
+// conv_geom of the pointwise descriptor, with the M tile fixed to one row of 128 tiles of one component
+static ConvGeom wino_geom(const dt_conv_desc* d) {
+  ConvGeom g = conv_geom(d, false);
+  g.ts = {1, d->Wi < 128 ? d->Wi : 128, 1, 1};
+  return g;
+}
+
+extern "C" int dt_wino_plan(int G, int Cin, int Cout, dt_conv_plan_t* o) {
+  DT_CHECK_ARG(o != nullptr, "dt_wino_plan: null pointer");
+  if (wino_check("dt_wino_plan", G, Cin, Cout)) return 1;
+  const dt_conv_desc d = wino_desc(G, Cin, Cout);
+  const ConvGeom g = wino_geom(&d);
+  memset(o, 0, sizeof(*o));
+  o->BN = g.BN; o->TH = g.ts.th; o->TW = g.ts.tw; o->TT = 1; o->TB = 1;
+  o->kiters = g.groups * g.nmma;
+  o->tiles = 16 * cdiv(G, g.ts.tw) * cdiv(Cout, g.BN);
+  o->useful_rows = (double)G / (cdiv(G, g.ts.tw) * 128.0);
+  plan_split<128>(g.groups, g.nmma, false, false, true, o);
+  o->mma_kblocks = (double)o->tiles * o->kiters;
+  return 0;
+}
+
+extern "C" int dt_wino_gemm(const void* v, const void* u, float* m, int G, int Cin, int Cout, void* stream_) {
+  if (wino_check("dt_wino_gemm", G, Cin, Cout)) return 1;
+  DT_CHECK_ARG(v && u && m, "dt_wino_gemm: null tensor pointer");
+  DT_CHECK_ARG(((uintptr_t)v % 16) == 0 && ((uintptr_t)u % 16) == 0 && ((uintptr_t)m % 16) == 0,
+               "dt_wino_gemm: tensors must be 16-byte aligned");
+  const dt_conv_desc d = wino_desc(G, Cin, Cout);
+  const ConvGeom g = wino_geom(&d);
+  const int TW = g.ts.tw;
+  ConvKernelParams p;
+  memset(&p, 0, sizeof(p));
+  p.N = 16; p.To = 1; p.Ho = 1; p.Wo = G; p.Cout = Cout;
+  p.kT = p.kH = p.kW = 1; p.sT = p.sH = p.sW = 1;
+  p.kchunks = g.kchunks;
+  p.TH = 1; p.TW = TW; p.TT = 1; p.TB = 1;
+  p.tiles_h = 1; p.tiles_w = cdiv(G, TW); p.tiles_t = 1; p.tiles_b = 16;
+  p.tiles_n = Cout / 128;
+  p.a_bytes = (uint32_t)TW * 128u;
+  p.out_f32 = 1;
+  p.split_in = 1;
+  p.ab_format = 1;
+  p.a_lo_off = Cin; p.b_lo_off = Cin;
+  p.Ti = 1; p.Hi = 1; p.Wi = G;
+  p.all_live = 1;
+  p.fd_n = make_fastdiv(p.tiles_n); p.fd_w = make_fastdiv(p.tiles_w); p.fd_h = make_fastdiv(1); p.fd_t = make_fastdiv(1);
+  p.total_tiles = 16 * p.tiles_w * p.tiles_n;
+  CUtensorMap tmA, tmB, tmC;
+  {
+    const uint64_t row = (uint64_t)2 * Cin * 2, comp = row * (uint64_t)G;
+    uint64_t dims[5] = {(uint64_t)2 * Cin, (uint64_t)G, 1, 1, 16};
+    uint64_t strides[4] = {row, comp, comp, comp};
+    uint32_t box[5] = {64, (uint32_t)TW, 1, 1, 1}, estr[5] = {1, 1, 1, 1, 1};
+    if (encode_map(&tmA, 0, 5, v, dims, strides, box, estr)) return 1;
+  }
+  {
+    uint64_t wd[3] = {(uint64_t)2 * Cin, (uint64_t)Cout, 16};
+    uint64_t ws[2] = {(uint64_t)2 * Cin * 2, (uint64_t)2 * Cin * 2 * Cout};
+    uint32_t wb[3] = {64, 128, 1}, we[3] = {1, 1, 1};
+    if (encode_map(&tmB, 0, 3, u, wd, ws, wb, we)) return 1;
+  }
+  if (encode_out_map(&tmC, m, 1, Cout, G, 1, 1, 16, Cout, g.ts)) return 1;
+  const int sms = num_sms();
+  const int grid = p.total_tiles < sms ? p.total_tiles : sms;
+  return launch_conv0<128, 0, false, 3, true, 0, true>(tmA, tmB, tmC, tmC, p, grid, (cudaStream_t)stream_);
 }
 
 

@@ -3,6 +3,8 @@ Tensors are NDHWC ([N, T, H, W, C], channels innermost); torch is only the memor
 container.  See include/dt_b200.h (dt_conv_desc / dt_conv3d) for the contract."""
 import ctypes as C
 
+import numpy as np
+
 from .. import _lib as L
 
 BF16, TF32 = 0, 1
@@ -153,6 +155,66 @@ def conv3d(x, w_packed, ksize, stride=(1, 1, 1), pad=(0, 0, 0), scale=None, bias
     L.call('dt_conv3d', C.byref(d), L.ptr(x), L.ptr(w_packed), L.ptr(scale), L.ptr(bias), L.ptr(residual),
            L.ptr(out), L.stream_ptr())
     return out.permute(1, 0, 2, 3, 4) if time_major else out
+
+
+# Winograd F(2x2, 3x3) of the bf16x3 keypoint head (include/dt_b200.h dt_wino_*): the 16 components xi = 4 i + j of a
+# 4 x 4 tile, V [16][G][2Cin] and U [16][Cout][2Cin] bf16 pairs, M [16][G][Cout] fp32, G = D * (S/2)^2 tiles.
+WINO_G = ((1.0, 0.0, 0.0), (0.5, 0.5, 0.5), (0.5, -0.5, 0.5), (0.0, 0.0, 1.0))
+
+
+def wino_filter(w):
+    """3x3 filter (Cout, Cin, [1,] 3, 3) -> U = G g G^T per (Cout, Cin), computed in fp64 and returned as fp32
+    [16, Cout, Cin] (numpy)."""
+    w = np.asarray(w, np.float64)
+    if w.ndim == 5:
+        assert w.shape[2] == 1
+        w = w[:, :, 0]
+    Cout, Cin = w.shape[:2]
+    assert w.shape[2:] == (3, 3)
+    Gm = np.asarray(WINO_G)
+    return np.einsum('ik,ockl,jl->ijoc', Gm, w, Gm).reshape(16, Cout, Cin).astype(np.float32)
+
+
+def pack_wino_weight(w):
+    """3x3 filter -> U as [16 (xi), Cout, 2 Cin] bf16 pairs [hi | lo] (the packed layout of a 16-tap conv)."""
+    torch = L.require_cuda()
+    return split_bf16(torch.from_numpy(wino_filter(w)).cuda())
+
+
+def wino_input(x, v):
+    """x [D, (1,) S, S, 2C] bf16 pairs -> V [16, D*(S/2)^2, 2C] (into v)."""
+    D, S, C2 = x.shape[0], x.shape[-2], x.shape[-1]
+    assert x.is_contiguous() and x.numel() == D * S * S * C2 and v.numel() == 16 * D * (S // 2) ** 2 * C2
+    L.call('dt_wino_input', L.ptr(x), D, S, C2 // 2, L.ptr(v), L.stream_ptr())
+    return v
+
+
+def wino_gemm(v, u, m, G):
+    """V [16, G, 2Cin], U [16, Cout, 2Cin] -> M [16, G, Cout] fp32 (into m)."""
+    _, Cout, C2 = u.shape
+    assert v.numel() == 16 * G * C2 and m.numel() == 16 * G * Cout and m.dtype == L.require_cuda().float32
+    L.call('dt_wino_gemm', L.ptr(v), L.ptr(u), L.ptr(m), G, C2 // 2, Cout, L.stream_ptr())
+    return m
+
+
+def wino_output_input(m, D, S, C, bias, relu, v):
+    """M [16, G, C] (+ bias, ReLU) -> the layer's bf16-pair output -> V of the next layer [16, G, 2C] (into v)."""
+    L.call('dt_wino_output_input', L.ptr(m), D, S, C, L.ptr(bias), int(bool(relu)), L.ptr(v), L.stream_ptr())
+    return v
+
+
+def wino_output(m, D, S, C, bias, relu, out):
+    """M [16, G, C] (+ bias, ReLU) -> out [D, (1,) S, S, 2C] bf16 pairs."""
+    assert out.is_contiguous() and out.numel() == D * S * S * 2 * C
+    L.call('dt_wino_output', L.ptr(m), D, S, C, L.ptr(bias), int(bool(relu)), L.ptr(out), L.stream_ptr())
+    return out
+
+
+def wino_plan(G, Cin, Cout):
+    """dt_wino_plan: the conv-kernel plan dt_wino_gemm launches (host only)."""
+    o = L.ConvPlan()
+    L.check(L.lib().dt_wino_plan(G, Cin, Cout, C.byref(o)), 'dt_wino_plan')
+    return o
 
 
 def pack_conv1_weight(w, dtype=BF16):

@@ -220,6 +220,20 @@ typedef struct dt_conv_plan_t {
 } dt_conv_plan_t;
 int dt_conv_plan(const dt_conv_desc* desc /*host*/, int residual_aligned, dt_conv_plan_t* plan /*host out*/);
 
+/* ---- Winograd F(2x2, 3x3) of the bf16x3 keypoint head (3x3, pad 1, stride 1 on S x S maps, S even) ----------------
+ * G = D * (S/2)^2 tiles.  V [16][G][2Cin] bf16 pairs (transformed input tiles, hi at c, lo at Cin + c), U [16][Cout][2Cin]
+ * bf16 pairs (transformed filters G g G^T, the packed layout of a 16-tap conv), M [16][G][Cout] fp32.
+ * dt_wino_gemm: M_xi = V_xi * U_xi^T for the 16 components xi in one launch of the conv kernel (split operands, three
+ * MMAs per k-block); Cin % 64 == 0, Cout % 128 == 0.  dt_wino_plan: its plan, host-only (no device work). */
+int dt_wino_gemm(const void* v, const void* u, float* m, int G, int Cin, int Cout, void* stream);
+int dt_wino_plan(int G, int Cin, int Cout, dt_conv_plan_t* plan /*host out*/);
+/* Transforms (wino.cu; C % 64 == 0, S even <= 16, D <= 65535).  x / y [D, S, S, 2C] bf16 pairs.
+ * dt_wino_input: x -> V.  dt_wino_output_input: M (+ bias [C] or NULL, ReLU if relu) -> the layer's bf16-pair output ->
+ * V of the next layer, without writing the output.  dt_wino_output: M (+ bias, ReLU) -> y. */
+int dt_wino_input(const void* x, int D, int S, int C, void* v, void* stream);
+int dt_wino_output_input(const float* m, int D, int S, int C, const float* bias, int relu, void* v, void* stream);
+int dt_wino_output(const float* m, int D, int S, int C, const float* bias, int relu, void* y, void* stream);
+
 /* conv1 of the ResNet bodies (lib/modeling/ResNet3D.py:258-261): 7x7 stride 2 pad 3 on the 3-channel
  * image + AffineChannel + ReLU, with the 7 taps of a filter row packed into one 128-byte k-block.
  * x_padded [F, 2, (Hp+6)/2, Wp+8, Cp] from dt_prep_clip(border 3, 4, row_planes 1), Cp*elemsize == 16;
