@@ -121,10 +121,11 @@ def conv_args(layer, mode):
             'f16': dict(dtype=2, x3=2, out_f32=0)}[mode]
 
 
-def step_plan(layer, mode, reduced=False):
+def step_plan(layer, mode, reduced=False, shapes=None):
+    """The plan of a table row at its step shape, or at its reduced shape in `shapes` (default REDUCED)."""
     name, N, T, H, W, Cin, Cout, k, s, p, rm = layer
     if reduced:
-        N, T, H, W = REDUCED[name]
+        N, T, H, W = (REDUCED if shapes is None else shapes)[name]
     return plan(N, T, H, W, Cin, Cout, k, s, p, res_mode=rm, **conv_args(layer, mode))
 
 

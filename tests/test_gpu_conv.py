@@ -342,16 +342,17 @@ def _epilogue(name):
     ReLU on the projection shortcut); everything else a bias, ReLU on the RPN / keypoint convs and the FCs."""
     if name.startswith('res'):
         return True, 'branch1' not in name
-    return False, name.startswith(('rpn conv', 'fc6', 'keypoint head'))
+    return False, name.startswith(('rpn conv', 'fc6', 'fc7', 'keypoint head'))
 
 
-def _step_inputs(layer, mode, g):
-    """Device tensors of one layer at its reduced shape, stored the way the engine stores them in `mode`, and the
-    values the kernel reads from them (rounded operands, hi + lo pairs, the stored residual) for the reference."""
+def _step_inputs(layer, mode, g, shapes=None):
+    """Device tensors of one layer at its reduced shape (in `shapes`, default REDUCED), stored the way the engine stores
+    them in `mode`, and the values the kernel reads from them (rounded operands, hi + lo pairs, the stored residual) for
+    the reference."""
     import torch
     from detectandtrack_b200.ops import conv as cv, dense_ops
     name, _, _, _, _, Cin, Cout, k, s, p, rm = layer
-    N, T, H, W = REDUCED[name]
+    N, T, H, W = (REDUCED if shapes is None else shapes)[name]
     To, Ho, Wo = (T + 2 * p[0] - k[0]) // s[0] + 1, (H + 2 * p[1] - k[1]) // s[1] + 1, (W + 2 * p[2] - k[2]) // s[2] + 1
     dt = cv.F16 if mode == 'f16' else cv.MODE_NAMES[mode]
     split = dt in cv.SPLIT_MODES
@@ -404,15 +405,20 @@ def test_step_layer_over_three_waves_vs_fp64(layer, mode, record_property):
     or more tiles per CTA, a ragged last wave) with the engine's storage and epilogue, against the fp64 tap-sum
     reference on the values the kernel reads.  bf16 outputs: |y - ref| <= 2^-8 |ref| + 2e-4 max|ref| elementwise (half a
     bf16 ulp of output rounding plus the accumulation-order error); the others _step_tol * max|ref|."""
+    _check_step_case(layer, mode, step_plan(layer, mode, reduced=True), None, '%s/%s' % (layer[0], mode), record_property)
+
+
+def _check_step_case(layer, mode, o, shapes, seed_tag, record_property):
+    """One table row at its reduced shape (`shapes`, default REDUCED; `o` its plan) through cv.conv3d, against conv_ref:
+    the body of test_step_layer_over_three_waves_vs_fp64, shared with tests/test_gpu_conv_workloads.py."""
     import zlib
     import torch
     from detectandtrack_b200.ops import conv as cv
     name, Cout = layer[0], layer[6]
-    o = step_plan(layer, mode, reduced=True)
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     assert o.tiles / sms >= 3, (name, mode, o.tiles, sms)
-    g = torch.Generator(device='cuda').manual_seed(zlib.crc32(('%s/%s' % (name, mode)).encode()))
-    run, ref_in = _step_inputs(layer, mode, g)
+    g = torch.Generator(device='cuda').manual_seed(zlib.crc32(seed_tag.encode()))
+    run, ref_in = _step_inputs(layer, mode, g, shapes)
     y = cv.conv3d(run['x'], run['w'], run['k'], run['s'], run['p'], run['scale'], run['bias'], run['res'], run['rm'],
                   run['relu'], out_f32=run['out_f32'], dtype=run['dtype'], out=run['out'], split_out=run['split_out'])
     if run['out'] is not None:
