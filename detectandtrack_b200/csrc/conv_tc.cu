@@ -144,7 +144,7 @@ struct ConvCfg {
   static constexpr int group_bytes(int nmma) { return boxes_a(nmma) * A_BYTES + boxes_b(nmma) * B_BYTES; }
   // K-heavy layers want a deep operand ring; K-light (HBM-bound) layers want output staging buffers so the
   // epilogue never waits for a TMA store to drain, and (with a residual) a ring of prefetched residual chunks.
-  static int tab_bytes(int groups) { return ((groups + 2) * 24 + 127) / 128 * 128; }   // schedule: one entry per group
+  static int tab_bytes(int groups) { return ((groups + 2) * 8 + 127) / 128 * 128; }    // schedule: one entry per group
   static void split(int groups, int nmma, bool res_tma, bool split_out, bool out_f32, int* stages, int* ks, int* ncbuf,
                     int* nrbuf) {
     const int kiters = groups * nmma;                   // MMA k-blocks per tile
@@ -160,9 +160,13 @@ struct ConvCfg {
     const int rb = split_out ? 2 * r : r;
     // with two split stages only one group's refill is in flight while the other's MMAs run, and a 64 KiB refill does
     // not land within one group's MMA time: a K-heavy split output is staged through one (hi, lo) slot pair instead of
-    // two when that buys a third stage (K-light layers measured faster with both slot pairs)
+    // two when that buys a third stage (K-light layers measured faster with both slot pairs).
+    // fp32-pair outputs (tf32x3) keep the split they had with 24-byte schedule entries, where the trade reached
+    // schedules of up to 110 groups: tests/test_conv_plan.py pins two slot pairs for the 216-group tf32x3 res4 3x3x3,
+    // although a third stage measured faster there too (DESIGN §5)
+    const bool f32_pairs_keep = split_out && out_f32 && groups > 110;
     const int st_wide = (fixed - (c + rb) * C_BYTES) / gb, st_lean = (fixed - (2 + rb) * C_BYTES) / gb;
-    if (split_out && nmma > 1 && c > 2 && kiters >= 12 && st_wide < 3 && st_lean > st_wide) c = 2;
+    if (split_out && nmma > 1 && c > 2 && kiters >= 12 && st_wide < 3 && st_lean > st_wide && !f32_pairs_keep) c = 2;
     // narrow tiles retire a k-block's MMAs faster than one producer / issuer round trip through the
     // mbarriers: let a ring stage carry two plain k-blocks there (same bytes in flight, half the handshakes)
     const int avail = fixed - (c + rb) * C_BYTES;
@@ -237,12 +241,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* c_free = r_full + 12;              // [4]       staging slot read out by its TMA store
   uint64_t* ml_ord = r_full + 16;              // [2]       consumer warpgroup g's mainloop has waited on all its ring stages
   uint64_t* ep_ord = r_full + 18;              // [2]       consumer warpgroup g's epilogue has staged all its chunks
-  // schedule of one tile, one entry per (tap, channel chunk) group: what the producers add to the tile's base
-  // coordinates for the group's first boxes (its lo boxes sit at the lo offsets from there).
-  // Built once; walking taps / channel chunks with carry logic in the producer loop costs more cycles per
-  // k-block than a narrow tile's MMAs take.
-  int4* tabA = reinterpret_cast<int4*>(reinterpret_cast<uint8_t*>(bars) + Cfg::BAR_BYTES);   // {c, dw, dh, dt}
-  int2* tabB = reinterpret_cast<int2*>(tabA + p.ktab);                                        // {c, weight block}
+  // schedule of one tile, one 8-byte entry per (tap, channel chunk) group: what the producers add to the tile's base
+  // coordinates for the group's first boxes (its lo boxes sit at the lo offsets from there), packed as
+  //   x = channel offset c (bits 0-15) | weight block (bits 16-31),   y = dw (bits 0-7) | dh (8-15) | dt (16-23)
+  // (launch_conv0 checks the ranges).  Both producer warps read the one entry.  Built once; walking taps / channel chunks
+  // with carry logic in the producer loop costs more cycles per k-block than a narrow tile's MMAs take.  The entry is
+  // kept small so that the tables of res5 3x3x3 (218 entries) and fc6 (198) leave room for a third 64 KiB split stage.
+  uint2* tab = reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(bars) + Cfg::BAR_BYTES);
   if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();
   {
     const int groups = p.kT * p.kH * p.kW * p.kchunks;
@@ -253,13 +258,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int kw = r % p.kW; r /= p.kW;
       const int kh = r % p.kH;
       const int kt = r / p.kH;
-      if (p.row_planes) {          // conv1: one box per filter row; split mode: weight blocks 2*kh (hi) and 2*kh + 1 (lo)
-        tabA[j] = make_int4(0, 0, kh >> 1, kh & 1);
-        tabB[j] = make_int2(0, tap * NB);
-      } else {
-        tabA[j] = make_int4(kc * BK, kw, kh, kt);
-        tabB[j] = make_int2(kc * BK, tap);
-      }
+      // conv1: one box per filter row; split mode: weight blocks 2*kh (hi) and 2*kh + 1 (lo)
+      const uint32_t c = p.row_planes ? 0u : (uint32_t)(kc * BK), blk = (uint32_t)(p.row_planes ? tap * NB : tap);
+      const uint32_t dw = p.row_planes ? 0u : (uint32_t)kw, dh = (uint32_t)(p.row_planes ? kh >> 1 : kh),
+                     dt = (uint32_t)(p.row_planes ? kh & 1 : kt);
+      tab[j] = make_uint2(c | blk << 16, dw | dh << 8 | dt << 16);
     }
   }
 
@@ -339,12 +342,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           int x0[2], x1[2], x2[2], x3[2];
 #pragma unroll
           for (int q = 0; q < 2; ++q) {
+            const uint2 e = tab[jq[q]];
+            x0[q] = (int)(e.x & 0xffffu);
             if (load_b) {
-              const int2 e = tabB[jq[q]];
-              x0[q] = e.x; x1[q] = n_base; x2[q] = WTAP ? e.y + n : e.y; x3[q] = 0;
+              const int blk = (int)(e.x >> 16);
+              x1[q] = n_base; x2[q] = WTAP ? blk + n : blk; x3[q] = 0;
             } else {
-              const int4 e = tabA[jq[q]];
-              x0[q] = e.x; x1[q] = w_base + e.y; x2[q] = h_base + e.z; x3[q] = t_base + e.w;
+              x1[q] = w_base + (int)(e.y & 0xffu); x2[q] = h_base + (int)((e.y >> 8) & 0xffu); x3[q] = t_base + (int)(e.y >> 16);
             }
           }
           mbar_wait_u(empty_u + stage * 8, phase ^ 1);
@@ -772,6 +776,7 @@ struct ConvGeom {
   bool res_up;                 // ... as the (TH/2 x TW/2) box of the coarser map of the FPN top-down add
   bool all_live;               // no tap is ever skipped (pointwise: the map is in output coordinates, without padding)
 };
+static double conv_mma_kblocks(const dt_conv_desc* d, const ConvGeom& g);
 static ConvGeom conv_geom(const dt_conv_desc* d, bool residual_aligned) {
   ConvGeom g;
   g.tf32 = d->dtype == DT_DTYPE_TF32;
@@ -780,10 +785,6 @@ static ConvGeom conv_geom(const dt_conv_desc* d, bool residual_aligned) {
   g.To = d->out_t_count > 0 ? d->out_t_count : g.To_full;
   g.Ho = (d->Hi + 2 * d->pH - d->kH) / d->sH + 1;
   g.Wo = (d->Wi + 2 * d->pW - d->kW) / d->sW + 1;
-  // stacking frames inside one TMA box needs unit temporal stride (pointwise convs fold strides into the map)
-  g.pointwise = d->kT == 1 && d->kH == 1 && d->kW == 1 && d->pT == 0 && d->pH == 0 && d->pW == 0;
-  g.ts = pick_tile(g.Ho, g.Wo, g.To, d->N, g.pointwise ? 256 : 256 / d->sW, g.pointwise ? 256 : 256 / d->sH,
-                   g.pointwise || d->sT == 1);
   // each consumer warpgroup keeps a 64 x BN fp32 accumulator in registers: BN / 2 per thread, so 128 is the widest
   // column tile that leaves the epilogue room under the 168-register cap of a 384-thread CTA
   g.BN = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : 32);
@@ -792,6 +793,20 @@ static ConvGeom conv_geom(const dt_conv_desc* d, bool residual_aligned) {
   g.kchunks = cdiv(d->Cin, g.BK);
   g.groups = d->kT * d->kH * d->kW * g.kchunks;
   g.nmma = g.split_in ? 3 : 1;                         // launch_conv: split operands take three products per group
+  // stacking frames inside one TMA box needs unit temporal stride (pointwise convs fold strides into the map)
+  g.pointwise = d->kT == 1 && d->kH == 1 && d->kW == 1 && d->pT == 0 && d->pH == 0 && d->pW == 0;
+  g.all_live = g.pointwise;
+  const int max_w = g.pointwise ? 256 : 256 / d->sW, max_h = g.pointwise ? 256 : 256 / d->sH;
+  g.ts = pick_tile(g.Ho, g.Wo, g.To, d->N, max_w, max_h, g.pointwise || d->sT == 1);
+  // Split operands: a stacked tile is kept only if it issues no more MMA k-blocks than the best unstacked one.  Every
+  // tile issues full 128-row MMAs, so the useful-row share pick_tile ranks by says little about the work, while a
+  // frame stack keeps every temporal tap live: res5 3x3x3 on 25 x 42 x 3 frames issues 657 k-blocks per clip and column
+  // tile as (1, 42) x 3 frames, 546 as (3, 42) x 1.  Plain operands keep pick_tile's choice.
+  if (g.nmma == 3 && (g.ts.tt > 1 || g.ts.tb > 1)) {
+    ConvGeom u = g;
+    u.ts = pick_tile(g.Ho, g.Wo, 1, 1, max_w, max_h, false);
+    if (conv_mma_kblocks(d, u) < conv_mma_kblocks(d, g)) g.ts = u.ts;
+  }
   // bf16 same-shape residual: its chunks are prefetched by TMA into a shared-memory ring (coalesced 128-byte
   // rows instead of 4-byte global loads per thread pair).
   // The FPN top-down add (res_mode 2) goes the same way when the tile is even-sized (tile origins are then even
@@ -799,7 +814,6 @@ static ConvGeom conv_geom(const dt_conv_desc* d, bool residual_aligned) {
   const bool res_even = (g.ts.th % 2 == 0) && (g.ts.tw % 2 == 0);
   g.res_tma = (d->res_mode == 1 || (d->res_mode == 2 && res_even)) && !d->out_f32 && !g.tf32 && residual_aligned;
   g.res_up = g.res_tma && d->res_mode == 2;
-  g.all_live = g.pointwise;
   return g;
 }
 
@@ -828,6 +842,9 @@ static int launch_conv0(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
   ConvKernelParams q = p;
   const int groups = p.kT * p.kH * p.kW * p.kchunks;
   DT_CHECK_ARG(groups <= 2048, "conv: %d (tap, channel chunk) groups per tile exceed the schedule table", groups);
+  DT_CHECK_ARG(p.kchunks * (KIND == 2 ? 32 : 64) <= 65536 && p.kT < 256 && p.kH < 256 && p.kW < 256,
+               "conv: channel offsets (%d chunks) or filter taps (%dx%dx%d) exceed the schedule entry", p.kchunks, p.kT,
+               p.kH, p.kW);
   Cfg::split(groups, NMMA, p.nrbuf > 0, p.split_out != 0, p.out_f32 != 0, &q.nstages, &q.ks, &q.ncbuf, &q.nrbuf);
   q.ktab = (groups + 2) & ~1;
   const int smem = Cfg::smem_bytes(groups, NMMA, q.nstages, q.ks, q.ncbuf, q.nrbuf, p.split_out != 0);

@@ -27,6 +27,7 @@ LAYERS = [
     ('res4 256>256 3x3x3', 3, 50, 84, 256, 256, (3, 3, 3), (1, 1, 1), (1, 1, 1)),
     ('res4 1024>256 1x1x1', 3, 50, 84, 1024, 256, (1, 1, 1), (1, 1, 1), (0, 0, 0)),
     ('res5 512>512 3x3x3', 3, 25, 42, 512, 512, (3, 3, 3), (1, 1, 1), (1, 1, 1)),
+    ('fpn_posthoc_P5 256>256 3x3x3', 3, 25, 42, 256, 256, (3, 3, 3), (1, 1, 1), (1, 1, 1)),
     ('fc6 12544>1024 (R=1000)', 1, 1, 1000, 12544, 1024, (1, 1, 1), (1, 1, 1), (0, 0, 0)),
     ('kps conv 512>512 3x3 (D=100)', 100, 14, 14, 512, 512, (1, 3, 3), (1, 1, 1), (0, 1, 1)),
 ]
