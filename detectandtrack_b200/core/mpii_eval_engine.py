@@ -6,11 +6,15 @@ the reference's ``core.mpii_eval_engine`` (lib/core/mpii_eval_engine.py):
     _run_posetrack_eval(roidb, det_file, dataset, output_dir)                 :246-314  (JSON writing part)
     run_mpii_eval(test_output_dir, roidb, dataset)                            :317-337
 
+    video2filenames(pathtodir)                                                :184-205
+    _run_eval(annot_dir, output_dir, eval_tracking, eval_pose)               :208-216
+
 What it does: per detection, remap the 17 COCO-order keypoints (x, y, logit) of ``detections_withTracks.pkl``
 to the 15 PoseTrack/MPII joints (neck = mid-shoulder, head_top = nose reflected about the neck), attach the
-track id and write one ``{'annolist': [...]}`` JSON per video.  The evaluation itself (the vendored ``poseval``
-package + the PoseTrack annotations) is outside the hot path; ``run_mpii_eval`` writes the files and calls the
-evaluator only if the caller hands one in.
+track id and write one ``{'annolist': [...]}`` JSON per video.  ``run_mpii_eval`` then scores the files: with an
+``evaluator`` handed in, by calling it; else, when the dataset has an ``annotation_directory`` (a dataset without
+one takes EVAL.POSETRACK_ANNOTATION_DIR), with the device PoseTrack evaluation (datasets/posetrack_eval.py), logging
+(total mAP, total MOTA) and, with EVAL.EVAL_MPII_PER_VIDEO, writing ``<det_file>_per_video_scores.txt``.
 
 Arithmetic note: the reference runs on numpy 1.14, where ``float32_scalar / 2.0`` and ``float32_scalar *
 python_float`` promote to float64.  The sums of two float32 values are therefore rounded in fp32 and everything
@@ -21,6 +25,7 @@ import logging
 import os
 import os.path as osp
 import pickle
+import time
 
 import numpy as np
 
@@ -155,6 +160,38 @@ def write_posetrack_json(roidb, dets, output_dir, image_directory='', out_filena
     return paths
 
 
+def video2filenames(pathtodir):
+    """:184-205.  {video directory: output JSON name} from the PoseTrack .mat annotations of ``pathtodir``."""
+    import scipy.io as sio
+    output = {}
+    for fname in os.listdir(pathtodir):
+        if not (osp.isfile(osp.join(pathtodir, fname)) and '.mat' in fname):
+            continue
+        data = sio.loadmat(osp.join(pathtodir, fname), squeeze_me=True, struct_as_record=False)
+        output[osp.dirname(data['annolist'][0].image.name)] = fname.replace('.mat', '.json')
+    return output
+
+
+def _run_eval(annot_dir, output_dir, eval_tracking=False, eval_pose=True, per_video=False):
+    """:208-216.  (total mAP, total MOTA) of the JSON files of ``output_dir`` against ``annot_dir``; with per_video
+    also {file name: (mAP, MOTA)} as each file scores on its own (NaN for both where that fails)."""
+    from ..datasets import posetrack_eval
+    res = posetrack_eval.evaluate(annot_dir, output_dir, eval_pose, eval_tracking,
+                                  cfg.TRACKING.DEBUG.UPPER_BOUND_4_EVAL_UPPER_BOUND, per_video=per_video)
+    (apAll, _, _), mota = res[0], res[1]
+    return (apAll[-1][0], mota[-4][0]) + tuple(res[2:])
+
+
+def _write_per_video_scores(path, paths, videos):
+    """:292-314: one 'video ap mota' line per video, sorted on the AP with Python's sorted."""
+    res = [(vname,) + tuple(videos.get(osp.basename(p), (np.nan, np.nan))) for vname, p in paths.items()]
+    res = sorted(res, key=lambda x: x[1])
+    logger.info('Writing per-video scores to %s', path)
+    with open(path, 'w') as fout:
+        for el in res:
+            fout.write('{} {} {}\n'.format(el[0], el[1], el[2]))
+
+
 def _run_posetrack_eval(roidb, det_file, dataset, output_dir, evaluator=None):
     with open(det_file, 'rb') as fin:
         try:
@@ -162,13 +199,30 @@ def _run_posetrack_eval(roidb, det_file, dataset, output_dir, evaluator=None):
         except UnicodeDecodeError:                       # pickles written by the py2 reference
             fin.seek(0)
             dets = pickle.load(fin, encoding='latin1')
-    image_directory = getattr(dataset, 'image_directory', '') if dataset is not None else ''
+    # a dataset without its own directories takes EVAL.POSETRACK_IMAGE_DIR / EVAL.POSETRACK_ANNOTATION_DIR ('' by default)
+    image_directory = getattr(dataset, 'image_directory', cfg.EVAL.POSETRACK_IMAGE_DIR) if dataset is not None else ''
     out_filenames = getattr(dataset, 'out_filenames', None) if dataset is not None else None
+    annot_dir = getattr(dataset, 'annotation_directory', cfg.EVAL.POSETRACK_ANNOTATION_DIR) if dataset is not None else ''
+    if evaluator is None and annot_dir and out_filenames is None and \
+            any(f.endswith('.mat') for f in os.listdir(annot_dir)):
+        out_filenames = video2filenames(annot_dir)
     paths = write_posetrack_json(roidb, dets, output_dir, image_directory, out_filenames)
-    if evaluator is None:
-        logger.info('No evaluator given: the PoseTrack evaluation (poseval + annotations) is outside this package')
+    if evaluator is not None:
+        return paths, evaluator(getattr(dataset, 'annotation_directory', None), output_dir, 'all_tracks' in dets)
+    if not annot_dir:
+        logger.info('No evaluator given and no annotation directory (EVAL.POSETRACK_ANNOTATION_DIR): '
+                    'the PoseTrack JSON files are written, not scored')
         return paths, None
-    return paths, evaluator(getattr(dataset, 'annotation_directory', None), output_dir, 'all_tracks' in dets)
+    eval_tracking = 'all_tracks' in dets
+    logger.info('Running dataset level evaluation...')
+    st_time = time.time()
+    res = _run_eval(annot_dir, output_dir, eval_tracking, per_video=cfg.EVAL.EVAL_MPII_PER_VIDEO)
+    logger.info('(total mAP, total MOTA) = %r', (float(res[0]), float(res[1])))
+    logger.info('...Done in %s', time.time() - st_time)
+    if cfg.EVAL.EVAL_MPII_PER_VIDEO:                     # every video scored alone, in the same device launches
+        _write_per_video_scores(osp.join(osp.dirname(osp.normpath(output_dir)), osp.basename(det_file) + '_per_video_scores.txt'),
+                                paths, res[2])
+    return paths, res[:2]
 
 
 def run_mpii_eval(test_output_dir, roidb, dataset=None, evaluator=None):

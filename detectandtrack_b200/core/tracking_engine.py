@@ -427,10 +427,10 @@ def compute_matches_tracks(json_data, dets, lstm_model=None):
     return dets
 
 
-def run_posetrack_tracking(test_output_dir, json_data, write_json=True):
+def run_posetrack_tracking(test_output_dir, json_data, write_json=True, dataset=None):
     """:758-795.  Writes detections_withTracks.pkl and then, like the reference's run_mpii_eval call
-    (:792-795), the per-video PoseTrack JSON files (core/mpii_eval_engine.py).  The evaluation itself
-    (vendored poseval + annotations) stays outside the package."""
+    (:792-795), the per-video PoseTrack JSON files (core/mpii_eval_engine.py).  With a dataset whose
+    annotation_directory is set (EVAL.POSETRACK_ANNOTATION_DIR), they are then scored against it."""
     det_file = cfg.TRACKING.DETECTIONS_FILE if len(cfg.TRACKING.DETECTIONS_FILE) else \
         osp.join(test_output_dir, 'detections.pkl')
     out_det_file = osp.join(test_output_dir, 'detections_withTracks.pkl')
@@ -450,5 +450,5 @@ def run_posetrack_tracking(test_output_dir, json_data, write_json=True):
     _write_det_file(dets_withTracks, out_det_file)
     if write_json:
         from . import mpii_eval_engine
-        mpii_eval_engine.run_mpii_eval(test_output_dir, json_data)
+        mpii_eval_engine.run_mpii_eval(test_output_dir, json_data, dataset)
     return dets_withTracks

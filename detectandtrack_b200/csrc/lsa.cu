@@ -4,18 +4,9 @@
 // The reference calls scipy.optimize.linear_sum_assignment (tracking_engine.py:237)
 // and accepts every pair.  Cost matrices here are ~90% exact ties (cost 1.0f for every
 // non-overlapping pair), so index parity needs the solver's visiting order, not just an
-// optimum: this kernel is a warp-parallel restatement of the rectangular shortest
-// augmenting path algorithm (Crouse 2016) in the exact order scipy >= 1.6 walks it
-// (see oracle/lsa.py, pinned live against the installed scipy):
-//   - fp64 duals / path costs, r = ((minVal + c) - u[i]) - v[j]        (no FMA possible)
-//   - remaining-column list filled in reverse, removal = swap with last
-//   - column choice: strict '<' keeps the FIRST minimum in list order, but an equal-cost
-//     UNASSIGNED column later in the list replaces it (so: last unassigned min if any,
-//     else first min)
-//   - nc < nr problems are solved on the transpose.
-// The 32 lanes split the remaining-column list (position it = lane, lane+32, ...); the
-// sequential rule above is reproduced by a (min, first-pos, last-unassigned-pos) reduction.
+// optimum: lsa_solver.cuh restates scipy's shortest augmenting path solver in its own order.
 #include "common.cuh"
+#include "lsa_solver.cuh"
 #include "../../include/dt_b200.h"
 #include <math_constants.h>
 
@@ -36,116 +27,13 @@ __device__ __forceinline__ float iou_pair_ref_l(const float* __restrict__ b, con
   return __fdiv_rn(inter, ua);
 }
 
-struct LsaSmem {
-  // carved from dynamic smem, sized for dmax
-  float* C;         // [nr*nc] internal (row-major, nr <= nc)
-  double* u;        // [dmax]
-  double* v;        // [dmax]
-  double* spc;      // [dmax]
-  int* path;        // [dmax]
-  int* col4row;     // [dmax]
-  int* row4col;     // [dmax]
-  int* remaining;   // [dmax]
-  unsigned char* SR;  // [dmax]
-  unsigned char* SC;  // [dmax]
-};
+// The tracker's cost matrices are float32 and sized for dmax x dmax.
+using LsaSmem = LsaSmemT<float>;
 
-__host__ __device__ inline size_t lsa_smem_bytes(int dmax) {
-  size_t b = 0;
-  b += (size_t)3 * dmax * sizeof(double);
-  b += (size_t)dmax * dmax * sizeof(float);
-  b += (size_t)4 * dmax * sizeof(int);
-  b += (size_t)2 * dmax;
-  return (b + 15) / 16 * 16;
-}
+__host__ __device__ inline size_t lsa_smem_bytes(int dmax) { return lsa_smem_bytes_t<float>(dmax, (size_t)dmax * dmax); }
 
 __device__ __forceinline__ LsaSmem lsa_carve(unsigned char* base, int dmax) {
-  LsaSmem s;
-  s.u = (double*)base;            base += (size_t)dmax * sizeof(double);
-  s.v = (double*)base;            base += (size_t)dmax * sizeof(double);
-  s.spc = (double*)base;          base += (size_t)dmax * sizeof(double);
-  s.C = (float*)base;             base += (size_t)dmax * dmax * sizeof(float);
-  s.path = (int*)base;            base += (size_t)dmax * sizeof(int);
-  s.col4row = (int*)base;         base += (size_t)dmax * sizeof(int);
-  s.row4col = (int*)base;         base += (size_t)dmax * sizeof(int);
-  s.remaining = (int*)base;       base += (size_t)dmax * sizeof(int);
-  s.SR = base;                    base += dmax;
-  s.SC = base;
-  return s;
-}
-
-// Solve on the internal (nr <= nc) matrix in s.C.  All 32 lanes participate.
-// On return col4row[i] (i < nr) holds the assignment.  Returns false if infeasible.
-__device__ bool lsa_solve_warp(const LsaSmem& s, int nr, int nc) {
-  const int lane = threadIdx.x & 31;
-  const unsigned FULL = 0xffffffffu;
-  for (int x = lane; x < nr; x += 32) { s.u[x] = 0.0; s.col4row[x] = -1; }
-  for (int x = lane; x < nc; x += 32) { s.v[x] = 0.0; s.row4col[x] = -1; s.path[x] = -1; }
-  __syncwarp();
-  for (int cur = 0; cur < nr; ++cur) {
-    for (int x = lane; x < nc; x += 32) { s.remaining[x] = nc - x - 1; s.spc[x] = CUDART_INF; s.SC[x] = 0; }
-    for (int x = lane; x < nr; x += 32) s.SR[x] = 0;
-    __syncwarp();
-    double minVal = 0.0;
-    int num_remaining = nc, sink = -1, i = cur;
-    while (sink == -1) {
-      if (lane == 0) s.SR[i] = 1;
-      const double ui = s.u[i];
-      const float* ci = s.C + (size_t)i * nc;
-      double lmin = CUDART_INF;
-      int lfirst = 0x7fffffff, lun = -1;
-      for (int it = lane; it < num_remaining; it += 32) {
-        const int j = s.remaining[it];
-        const double r = __dsub_rn(__dsub_rn(__dadd_rn(minVal, (double)ci[j]), ui), s.v[j]);
-        double sp = s.spc[j];
-        if (r < sp) { s.path[j] = i; s.spc[j] = r; sp = r; }
-        const bool un = (s.row4col[j] == -1);
-        if (sp < lmin) { lmin = sp; lfirst = it; lun = un ? it : -1; }
-        else if (sp == lmin && un) { lun = it; }
-      }
-      double m = lmin;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) m = fmin(m, __shfl_xor_sync(FULL, m, o));
-      if (m == CUDART_INF) return false;              // infeasible (cannot happen for finite costs)
-      int f = (lmin == m) ? lfirst : 0x7fffffff;
-      int un = (lmin == m) ? lun : -1;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        f = min(f, __shfl_xor_sync(FULL, f, o));
-        un = max(un, __shfl_xor_sync(FULL, un, o));
-      }
-      const int index = (un >= 0) ? un : f;
-      minVal = m;
-      const int j = s.remaining[index];
-      const int r4c = s.row4col[j];
-      if (r4c == -1) sink = j; else i = r4c;
-      --num_remaining;
-      __syncwarp();
-      if (lane == 0) { s.SC[j] = 1; s.remaining[index] = s.remaining[num_remaining]; }
-      __syncwarp();
-    }
-    // dual update (rectangular_lsap: "update dual variables")
-    if (lane == 0) s.u[cur] = __dadd_rn(s.u[cur], minVal);
-    for (int x = lane; x < nr; x += 32)
-      if (s.SR[x] && x != cur) s.u[x] = __dadd_rn(s.u[x], __dsub_rn(minVal, s.spc[s.col4row[x]]));
-    for (int x = lane; x < nc; x += 32)
-      if (s.SC[x]) s.v[x] = __dsub_rn(s.v[x], __dsub_rn(minVal, s.spc[x]));
-    __syncwarp();
-    // augment along the path
-    if (lane == 0) {
-      int j = sink;
-      while (true) {
-        const int ii = s.path[j];
-        s.row4col[j] = ii;
-        const int tmp = s.col4row[ii];
-        s.col4row[ii] = j;
-        j = tmp;
-        if (ii == cur) break;
-      }
-    }
-    __syncwarp();
-  }
-  return true;
+  return lsa_carve_t<float>(base, dmax, (size_t)dmax * dmax);
 }
 
 // mode 0: cost given  [B, pmax, ldc] (rows = prev, cols = cur), per-problem (nprev, ncur)

@@ -609,6 +609,44 @@ int dt_flow_smooth_poses(const float* poses, const float* boxes, const int* coun
                          const unsigned char* no_flow, int n_context, const int* out_tracks, const int* out_counts, int omax,
                          float* out_poses, float* out_boxes, void* stream);
 
+
+/* ---- poseval.cu: PoseTrack evaluation (lib/datasets/posetrack/poseval/py/evaluate_simple.py) ---------------------- */
+
+#define DT_PT_JOINTS 15             /* PoseTrack / MPII joints (eval_helpers.Joint) */
+#define DT_PT_MAX_GT 64             /* GT people per frame */
+#define DT_PT_MAX_MAP_IDS 4096      /* distinct GT track ids one CLEAR-MOT frame list may see */
+
+/* assignGTmulti (eval_helpers.py:423-637) for every frame, one CTA per frame.  Frame f owns GT rows
+ * [gt_off[f], gt_off[f+1]) and prediction rows [pr_off[f], pr_off[f+1]) (at most max_gt <= DT_PT_MAX_GT and
+ * max_pr <= DT_LSA_MAX_DIM of them); pair_off [nframes] = sum over earlier frames of (predictions x GT).
+ * gt_rect [NG, 4] fp64 head box (x1, y1, x2, y2); gt_kp [NG, 15, 3] fp64 (x, y, present); pr_kp [NP, 15, 4] fp64
+ * (x, y, score, present).  Outputs: labels [NP, 15] (-1: joint not predicted, else the AP label 0 / 1); ngt [15, nframes]
+ * annotated GT joints; dist [pair_off[F], 15] fp64: the distance of (prediction p, GT g, joint j) of frame f at
+ * (pair_off[f] + p * nG + g) * 15 + j where it matches (<= 0.5), NaN elsewhere (only frames with both are written). */
+int dt_posetrack_assign(const int* gt_off, const int* pr_off, const long long* pair_off, int nframes, const double* gt_rect,
+                        const double* gt_kp, const double* pr_kp, int max_gt, int max_pr, signed char* labels, int* ngt,
+                        double* dist, void* stream);
+/* Workspace of dt_posetrack_ap for nentries scores in all. */
+int dt_posetrack_ap_workspace_bytes(long long nentries, size_t* bytes /*host out*/);
+/* evaluateAP.computeMetrics (computeRPC + VOCap) of every segment: segs [nseg, 3] = (joint, first frame, end frame),
+ * the scores of that joint's predicted rows of those frames, placed at seg_off [nseg + 1] (nentries = seg_off[nseg]).
+ * Scores are sorted descending, ties by row (the reference's concatenation order).  out [nseg, 3] fp64 = (AP, last
+ * precision, last recall) x 100, zero for an empty segment; IEEE 0/0 where the joint has no GT. */
+int dt_posetrack_ap(const double* pr_kp, const signed char* labels, const int* ngt, int nframes, const int* pr_off,
+                    const int* segs, const int* seg_off, int nseg, long long nentries, double* out, void* workspace,
+                    size_t workspace_bytes, void* stream);
+/* Dynamic shared memory of one dt_posetrack_mot warp (the caller checks it against the device's 227 KB). */
+int dt_posetrack_mot_smem_bytes(int max_gt, int max_pr, int map_cap, size_t* bytes /*host out*/);
+/* MOTAccumulator.update (py-motmetrics mot.py:90-191) over frame lists, one warp per (list, joint): list l feeds update()
+ * the MOT inputs of frames list_frames[list_off[l] .. list_off[l+1]) in order, built from dt_posetrack_assign's dist and
+ * the rows that have the joint (track ids gt_tid [NG], pr_tid [NP]).  max_gt / max_pr bound those rows per frame and
+ * joint, map_cap the distinct GT track ids of a list.  Outputs: counts [nlists, 15, 4] int32 = MATCH, SWITCH, FP, MISS;
+ * sumd [nlists, 15] fp64 = sum of the MATCH / SWITCH distances; status [nlists * 15] (may be NULL) non-zero where a bound
+ * was exceeded. */
+int dt_posetrack_mot(const int* gt_off, const int* pr_off, const long long* pair_off, const double* gt_kp, const int* gt_tid,
+                     const double* pr_kp, const int* pr_tid, const double* dist, const int* list_off, const int* list_frames,
+                     int nlists, int max_gt, int max_pr, int map_cap, int* counts, double* sumd, int* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -3,7 +3,8 @@
 
     python tools/compute_tracks.py --cfg X.yaml [KEY VALUE ...]
 Loads <output_dir>/detections.pkl (or TRACKING.DETECTIONS_FILE), links detections per video
-on the GPU and writes detections_withTracks.pkl."""
+on the GPU and writes detections_withTracks.pkl and the PoseTrack JSON of every video; with
+EVAL.POSETRACK_ANNOTATION_DIR set, scores them (total mAP and MOTA) on the GPU."""
 import argparse
 import logging
 import os
@@ -30,8 +31,8 @@ def main():
         cfg_from_list(args.opts)
     assert_and_infer_cfg()
     test_output_dir = get_output_dir(training=False)
-    json_data, _, _, _, _ = get_roidb_and_dataset(None, include_gt=True)
-    run_posetrack_tracking(test_output_dir, json_data)
+    json_data, dataset, _, _, _ = get_roidb_and_dataset(None, include_gt=True)
+    run_posetrack_tracking(test_output_dir, json_data, dataset=dataset)
 
 
 if __name__ == '__main__':
