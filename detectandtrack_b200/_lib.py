@@ -100,7 +100,11 @@ HOST_FUNCS = {'dt_planes_ld': ([_i, _i, _i, _i], C.c_int), 'dt_jpeg_available': 
               'dt_posetrack_ap_workspace_bytes': ([C.c_longlong, C.POINTER(_sz)], C.c_int),
               'dt_posetrack_ap': ([_p, _p, _p, _i, _p, _p, _p, _i, C.c_longlong, _p, _p, _sz, _p], C.c_int),
               'dt_posetrack_mot_smem_bytes': ([_i, _i, _i, C.POINTER(_sz)], C.c_int),
-              'dt_posetrack_mot': ([_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _p], C.c_int)}
+              'dt_posetrack_mot': ([_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _p], C.c_int),
+              'dt_posetrack_upper_bound': ([_p, _p, _p, _i, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p], C.c_int),
+              # TRACKING.DEBUG.UPPER_BOUND* kernels: launchers too, with their argument-error cases in tests/test_upper_bound.py
+              'dt_gt_frame_costs': ([_p, _i, _i, _p, _i, _i, _i, _i, C.c_double, _p, _i, _i, _f, C.c_double, _p, _p], C.c_int),
+              'dt_track_upper_bound': ([_p, _i, _p, _i, _i, _p, _p, _i, _i, _p, _i, _p, _i, _i, _p, _p, _p, _p, _p], C.c_int)}
 SOFT_NMS_METHODS = {'hard': 0, 'linear': 1, 'gaussian': 2}     # DT_SOFT_NMS_* of include/dt_b200.h
 FARNEBACK_GAUSSIAN = 256           # DT_FARNEBACK_GAUSSIAN of include/dt_b200.h (cv2.OPTFLOW_FARNEBACK_GAUSSIAN)
 FLOW_MAX_CONTEXT = 16              # DT_FLOW_MAX_CONTEXT of include/dt_b200.h
@@ -110,6 +114,7 @@ LSA_MAX_DIM = 224                   # DT_LSA_MAX_DIM of include/dt_b200.h
 PT_JOINTS = 15                      # DT_PT_JOINTS of include/dt_b200.h
 PT_MAX_GT = 64                      # DT_PT_MAX_GT of include/dt_b200.h
 PT_MAX_MAP_IDS = 4096               # DT_PT_MAX_MAP_IDS of include/dt_b200.h
+UB_COMPACT, UB_GT_KPS, UB_ONLY_CONF = 1, 2, 4   # DT_UB_* of include/dt_b200.h
 
 
 

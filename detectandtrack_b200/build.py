@@ -20,7 +20,7 @@ ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr',
           '-I' + os.path.join(ROOT, 'include')]
 # bit-exact integer/index kernels: no FMA contraction anywhere in these units
-EXACT = {'boxes.cu', 'lsa.cu', 'proposals.cu', 'detections.cu', 'targets.cu', 'flow.cu', 'poseval.cu'}
+EXACT = {'boxes.cu', 'lsa.cu', 'proposals.cu', 'detections.cu', 'targets.cu', 'flow.cu', 'poseval.cu', 'upper_bound.cu'}
 
 
 def _newer(src, dst, extra=()):

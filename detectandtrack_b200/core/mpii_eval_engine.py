@@ -176,8 +176,8 @@ def _run_eval(annot_dir, output_dir, eval_tracking=False, eval_pose=True, per_vi
     """:208-216.  (total mAP, total MOTA) of the JSON files of ``output_dir`` against ``annot_dir``; with per_video
     also {file name: (mAP, MOTA)} as each file scores on its own (NaN for both where that fails)."""
     from ..datasets import posetrack_eval
-    res = posetrack_eval.evaluate(annot_dir, output_dir, eval_pose, eval_tracking,
-                                  cfg.TRACKING.DEBUG.UPPER_BOUND_4_EVAL_UPPER_BOUND, per_video=per_video)
+    run = posetrack_eval.evaluate_upper_bound if cfg.TRACKING.DEBUG.UPPER_BOUND_4_EVAL_UPPER_BOUND else posetrack_eval.evaluate
+    res = run(annot_dir, output_dir, eval_pose, eval_tracking, per_video=per_video)
     (apAll, _, _), mota = res[0], res[1]
     return (apAll[-1][0], mota[-4][0]) + tuple(res[2:])
 

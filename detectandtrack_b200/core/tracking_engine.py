@@ -16,6 +16,10 @@ Only the 'bbox-overlap' cost runs on the device (the configuration of every ship
 weights of the other costs are 0, config.py:550-551), with 'hungarian' or 'greedy' matching;
 anything else raises NotImplementedError.
 
+TRACKING.DEBUG.UPPER_BOUND / _2_GT_KPS / _5_GT_KPS_ONLY (:282-338), the upper-bound experiments, match the GT of every frame
+against its detections in one batched pass over the frames interleaved with their GT (csrc/upper_bound.cu), then one
+launch keeps the matched detections with the GT's track ids and copies the GT's boxes and keypoints onto them.
+
 TRACKING.FLOW_SMOOTHING_ON (:401-643) runs after the id pass, one video at a time: Farneback flow
 between consecutive key frames (csrc/flow.cu, all pairs of a frame size in one call), the shot-boundary
 test np.abs(flow).mean() > FLOW_SHOT_BOUNDARY_TH on the device, then one launch that shifts every pose
@@ -202,10 +206,19 @@ def _compute_matches(prev_frame_data, cur_frame_data, prev_boxes, cur_boxes,
     return m[1, :nboxes].cpu().numpy().astype(np.int32)
 
 
-def _tracks_for_videos(videos_boxes, videos_poses=None, kpt_names=None):
+def _pose_cost_args(videos_poses, kpt_names=None):
+    names = list(kpt_names or POSETRACK_KEYPOINTS)
+    K = cfg.KRCNN.NUM_KEYPOINTS
+    if K <= 0:                                   # unset (config default -1): take it from the data
+        K = next((np.asarray(p).shape[-1] for vp in videos_poses for fr in vp for p in (fr or [])), len(names))
+    return K, names.index('head_top'), names.index('head_bottom')
+
+
+def _tracks_for_videos(videos_boxes, videos_poses=None, kpt_names=None, videos_prev_poses=None):
     """videos_boxes: list (videos) of lists (frames) of (n,4T+1) arrays; videos_poses (needed when the 'pose-pck' cost is
-    active): same nesting of lists of [4, K] keypoint arrays.  Returns list of list of python-int id lists, one batched
-    device pass."""
+    active): same nesting of lists of [4, K] keypoint arrays.  videos_prev_poses (same nesting, or None): the poses frame f
+    shows as the previous frame of f + 1 when they differ from its own (UPPER_BOUND_5_GT_KPS_ONLY replaces them after the
+    match, :325-338).  Returns list of list of python-int id lists, one batched device pass."""
     import torch
     flat, first = [], []
     for vb in videos_boxes:
@@ -225,16 +238,15 @@ def _tracks_for_videos(videos_boxes, videos_poses=None, kpt_names=None):
     d_start = torch.from_numpy(is_start).cuda()
     if w_pck == 0.0:
         matches, _ = box_ops.match_frames(torch.from_numpy(packed).cuda(), d_counts, d_start, T=T, weight=w_iou, algo=algo)
+    elif videos_prev_poses is not None:
+        matches = _pair_matches(flat, first, videos_poses, videos_prev_poses, packed.shape[1], w_iou, w_pck, algo, kpt_names)
     else:
         # combined cost (tracking_engine.py:158-181): cost matrices of every frame pair in one launch, then the batched solver
         assert videos_poses is not None, "the 'pose-pck' cost needs the poses of every detection"
-        names = list(kpt_names or POSETRACK_KEYPOINTS)
-        K = cfg.KRCNN.NUM_KEYPOINTS
-        if K <= 0:                                   # unset (config default -1): take it from the data
-            K = next((np.asarray(p).shape[-1] for vp in videos_poses for fr in vp for p in (fr or [])), len(names))
+        K, ht, hb = _pose_cost_args(videos_poses, kpt_names)
         poses = _pack_poses([p for vp in videos_poses for p in vp], packed.shape[1], K)
         cost = box_ops.frame_costs(torch.from_numpy(packed).cuda(), d_counts, d_start, torch.from_numpy(poses).cuda(), T=T, w_iou=w_iou,
-                                   w_pck=w_pck, head_top=names.index('head_top'), head_bottom=names.index('head_bottom'))
+                                   w_pck=w_pck, head_top=ht, head_bottom=hb)
         nrows = torch.cat([d_counts[:1] * 0, d_counts[:-1]]) * (1 - d_start.to(torch.int32))
         matches, status = box_ops.lsa_batched(cost, nrows, d_counts, algo)
     tracks = box_ops.assign_track_ids(matches, d_counts, torch.tensor(first, dtype=torch.int32), d_start)
@@ -246,23 +258,189 @@ def _tracks_for_videos(videos_boxes, videos_poses=None, kpt_names=None):
     return out
 
 
+def _pair_matches(flat, first, videos_poses, videos_prev_poses, dmax, w_iou, w_pck, algo, kpt_names=None):
+    """The combined cost of every frame pair (f - 1, f) of every video with frame f - 1's poses taken from
+    videos_prev_poses: the pairs are packed pair-interleaved, [(f - 1, f), ...] with is_start on every first entry, for
+    dt_frame_costs + dt_lsa_batched.  Returns matches [F, dmax] in frame order (first frames of videos: -1)."""
+    import torch
+    F = len(flat)
+    cur = [p for vp in videos_poses for p in vp]
+    prev = [p for vp in videos_prev_poses for p in vp]
+    is_first = np.zeros(F, dtype=bool)
+    is_first[np.array(first, dtype=np.int64)] = True
+    pair_of = [f for f in range(F) if not is_first[f]]
+    out = torch.full((F, dmax), -1, dtype=torch.int32, device='cuda')
+    if not pair_of:
+        return out
+    boxes, pposes = [], []
+    for f in pair_of:
+        boxes += [flat[f - 1], flat[f]]
+        pposes += [prev[f - 1], cur[f]]
+    packed, counts = _pack(boxes)
+    T = (packed.shape[2] - 1) // 4
+    K, ht, hb = _pose_cost_args([pposes], kpt_names)
+    poses = _pack_poses(pposes, packed.shape[1], K)
+    is_start = np.zeros(len(boxes), dtype=np.uint8)
+    is_start[0::2] = 1
+    d_counts = torch.from_numpy(counts).cuda()
+    cost = box_ops.frame_costs(torch.from_numpy(packed).cuda(), d_counts, torch.from_numpy(is_start).cuda(),
+                               torch.from_numpy(poses).cuda(), T=T, w_iou=w_iou, w_pck=w_pck, head_top=ht, head_bottom=hb)
+    nrows = torch.cat([d_counts[:1] * 0, d_counts[:-1]]) * (1 - torch.from_numpy(is_start).cuda().to(torch.int32))
+    m, _ = box_ops.lsa_batched(cost, nrows, d_counts, algo)
+    w = min(dmax, m.shape[1])
+    out[torch.tensor(pair_of, device='cuda'), :w] = m[1::2, :w]
+    return out
+
+
+# ------------------------------------------------------------------------------ upper-bound experiments
+def _gt_arrays(entry, i, T):
+    """The GT of a roidb entry as the reference's roidb holds it: boxes [G, 4T] fp32, gt_keypoints [G, 3, K] int32 (json_dataset
+    stores the annotation's coordinates in an int32 array, truncating them; a JSON-list roidb hands them over as they are in
+    the file), tracks [G]."""
+    for k in ('boxes', 'gt_keypoints', 'tracks'):
+        if k not in entry:
+            raise ValueError("TRACKING.DEBUG.UPPER_BOUND*: roidb entry %d (%s) has no ground truth '%s'" % (i, _image_path(entry), k))
+    boxes = np.asarray(entry['boxes'], dtype=np.float32)
+    boxes = boxes.reshape(-1, boxes.shape[-1]) if boxes.size else np.zeros((0, 4 * T), np.float32)
+    kps = np.asarray(entry['gt_keypoints']).astype(np.int32)
+    tracks = np.asarray(entry['tracks']).reshape(-1)
+    if len(tracks) != len(boxes) or (kps.size and kps.shape[0] != len(boxes)):
+        raise ValueError('roidb entry %d: %d GT boxes, %d keypoint sets and %d track ids' % (i, len(boxes), len(kps), len(tracks)))
+    if boxes.shape[1] != 4 * T:
+        raise NotImplementedError('TRACKING.DEBUG.UPPER_BOUND*: roidb entry %d has GT boxes of %d columns for detections of '
+                                  '%d frame(s)' % (i, boxes.shape[1], T))
+    return boxes, kps, tracks
+
+
+def _box_frames(dets):
+    """T of the detections (4T + 1 box columns)."""
+    ld = next((np.shape(b)[-1] for b in dets['all_boxes'][1] if len(b)), 5)
+    return (ld - 1) // 4
+
+
+def _check_upper_bound_options(json_data=None, dets=None):
+    """Rejects, before any device work, the upper-bound modes the device path does not run and a roidb without the GT
+    they read."""
+    dbg = cfg.TRACKING.DEBUG
+    if dbg.UPPER_BOUND_3_SHOTS:
+        raise NotImplementedError('TRACKING.DEBUG.UPPER_BOUND_3_SHOTS reads a hard-coded shot-boundary file '
+                                  '(/path/to/shot_boundaries_val.csv, :258-271) that is not part of the release')
+    if not (dbg.UPPER_BOUND or dbg.UPPER_BOUND_5_GT_KPS_ONLY) or json_data is None:
+        return
+    T = _box_frames(dets)
+    if dbg.UPPER_BOUND and dbg.UPPER_BOUND_2_GT_KPS and T > 1:
+        raise NotImplementedError('TRACKING.DEBUG.UPPER_BOUND_2_GT_KPS sets new_boxes[:, :4] from the GT (:313), which '
+                                  'takes centre-frame boxes (T = 1); the detections have T = %d' % T)
+    for i, entry in enumerate(json_data):
+        _gt_arrays(entry, i, T)
+
+
+def _upper_bound_tracks(all_video_roidb, dets):
+    """:282-338 for every video in one batched device pass.  Replaces the boxes / poses of dets as the reference does and
+    returns the per-video lists of per-frame id lists (the GT track ids under UPPER_BOUND, else the regular id pass over
+    the frames, with the _5 poses of frame f - 1 in the pose-pck cost of the pair (f - 1, f))."""
+    import torch
+    dbg = cfg.TRACKING.DEBUG
+    ub, ub2, conf_only, ub5 = dbg.UPPER_BOUND, dbg.UPPER_BOUND_2_GT_KPS, dbg.UPPER_BOUND_2_GT_KPS_ONLY_CONF, dbg.UPPER_BOUND_5_GT_KPS_ONLY
+    frames = [e for v in all_video_roidb for e in v]
+    F = len(frames)
+    if F == 0:
+        return [[] for _ in all_video_roidb]
+    boxes = [_get_boxes(dets, det_id) for (_, det_id) in frames]
+    poses = [_get_poses(dets, det_id) for (_, det_id) in frames]
+    T = _box_frames(dets)
+    ld = 4 * T + 1
+    w_iou, w_pck = _cost_weights(cfg.TRACKING.DISTANCE_METRICS, cfg.TRACKING.DISTANCE_METRIC_WTS)
+    algo = cfg.TRACKING.BIPARTITE_MATCHING_ALGO
+    if algo not in box_ops.ALGOS:
+        raise NotImplementedError('Unknown matching algo: {}'.format(algo))
+    gts = [_gt_arrays(e, det_id, T) for (e, det_id) in frames]
+    stacked = [np.stack(ps).astype(np.float32, copy=False) if len(ps) else None for ps in poses]
+    shapes = {p.shape[1:] for p in stacked if p is not None}
+    if len(shapes) > 1:
+        raise NotImplementedError('detection poses of different shapes: %s' % sorted(shapes))
+    R, K = shapes.pop() if shapes else (4, max([g[1].shape[-1] for g in gts if g[1].size] + [17]))
+    if R < 3:
+        raise NotImplementedError('detection poses of %d rows: the GT replaces rows 0..2' % R)
+    for i, (_, kp, _) in enumerate(gts):
+        if kp.size and kp.shape[1:] != (3, K):
+            raise NotImplementedError('roidb entry %d: GT keypoints %s for detection poses [%d, %d]'
+                                      % (frames[i][1], kp.shape, R, K))
+    dmax = max([len(b) for b in boxes] + [len(g[0]) for g in gts] + [1])
+    if dmax > box_ops.L.LSA_MAX_DIM:
+        raise ValueError('TRACKING.DEBUG.UPPER_BOUND*: %d GT people or detections in a frame (at most %d)'
+                         % (dmax, box_ops.L.LSA_MAX_DIM))
+    pb = np.zeros((2 * F, dmax, ld), np.float32)
+    pp = np.zeros((2 * F, dmax, R, K), np.float32)
+    cnt = np.zeros(2 * F, np.int32)
+    tid = np.full((F, dmax), -1, np.int32)
+    for f in range(F):
+        gb, gk, gt = gts[f]
+        cnt[2 * f], cnt[2 * f + 1] = len(gb), len(boxes[f])
+        pb[2 * f, :len(gb), :4 * T] = gb
+        if gk.size:
+            pp[2 * f, :len(gk), :3] = gk
+        tid[f, :len(gt)] = gt
+        if len(boxes[f]):
+            pb[2 * f + 1, :len(boxes[f])] = boxes[f]
+        if stacked[f] is not None:
+            pp[2 * f + 1, :len(stacked[f])] = stacked[f]
+    is_start = np.zeros(2 * F, np.uint8)
+    is_start[0::2] = 1
+    d_b, d_p, d_n = torch.from_numpy(pb).cuda(), torch.from_numpy(pp).cuda(), torch.from_numpy(cnt).cuda()
+    d_s = torch.from_numpy(is_start).cuda()
+    matches = matches_gt = None
+    if ub:
+        if w_pck == 0.0:
+            matches, _ = box_ops.match_frames(d_b, d_n, d_s, T=T, weight=w_iou, algo=algo)
+        else:
+            _, ht, hb = _pose_cost_args([poses])
+            cost = box_ops.gt_frame_costs(d_b, d_n, d_p, T=T, w_iou=w_iou, w_pck=w_pck, head_top=ht, head_bottom=hb)
+            matches, _ = box_ops.lsa_batched(cost, d_n[0::2], d_n[1::2], algo)
+    if ub5:                                                   # bbox-overlap, weight 1, hungarian (:329-333)
+        matches_gt, _ = box_ops.match_frames(d_b, d_n, d_s, T=T, weight=1.0, algo='hungarian')
+    flags = (box_ops.L.UB_COMPACT if ub else 0) | (box_ops.L.UB_GT_KPS if ub and ub2 else 0) | \
+        (box_ops.L.UB_ONLY_CONF if ub and ub2 and conf_only else 0)
+    ob, op, ot, on = box_ops.track_upper_bound(d_b, d_p, d_n, torch.from_numpy(tid).cuda(), matches, matches_gt, flags)
+    ob, op, ot, on = ob.cpu().numpy(), op.cpu().numpy(), ot.cpu().numpy(), on.cpu().numpy()
+    new_poses = []
+    for f, (_, det_id) in enumerate(frames):
+        n = int(on[f])
+        dets['all_boxes'][1][det_id] = ob[f, :n].copy()
+        new_poses.append(list(op[f, :n].copy()))
+        dets['all_keyps'][1][det_id] = new_poses[-1]
+    out, f0 = [], 0
+    if ub:
+        for v in all_video_roidb:
+            out.append([ot[f, :int(on[f])].tolist() for f in range(f0, f0 + len(v))])
+            f0 += len(v)
+        return out
+    vb, vp, vq = [], [], []
+    for v in all_video_roidb:
+        vb.append(boxes[f0:f0 + len(v)]); vp.append(poses[f0:f0 + len(v)]); vq.append(new_poses[f0:f0 + len(v)])
+        f0 += len(v)
+    return _tracks_for_videos(vb, vp, videos_prev_poses=vq)
+
+
 def _compute_tracks_video(video_json_data, dets):
-    """:272-350 (non-debug path) for one video: list of per-frame id lists."""
-    if (cfg.TRACKING.DEBUG.UPPER_BOUND or cfg.TRACKING.DEBUG.UPPER_BOUND_3_SHOTS or
-            cfg.TRACKING.DEBUG.UPPER_BOUND_5_GT_KPS_ONLY):
-        raise NotImplementedError('TRACKING.DEBUG.* upper-bound modes are not on the device path')
+    """:272-350 for one video: list of per-frame id lists (the TRACKING.DEBUG.UPPER_BOUND* modes replace the video's
+    boxes and poses in dets, as the reference does)."""
+    _check_upper_bound_options([e for e, _ in video_json_data], dets)
+    if cfg.TRACKING.DEBUG.UPPER_BOUND or cfg.TRACKING.DEBUG.UPPER_BOUND_5_GT_KPS_ONLY:
+        return _upper_bound_tracks([video_json_data], dets)[0]
     boxes = [_get_boxes(dets, det_id) for (_, det_id) in video_json_data]
     poses = [_get_poses(dets, det_id) for (_, det_id) in video_json_data]
     return _tracks_for_videos([boxes], [poses])[0]
 
 
 # ------------------------------------------------------------------------------ flow smoothing
-def _check_tracking_options(dets):
+def _check_tracking_options(dets, json_data=None):
     """Rejects, before any device work, what the device path does not run: LSTM tracking, and flow smoothing with
     anything but centre-frame boxes (T = 1) and [4, 17] poses (the shapes _weighted_avg_poses and _combine_boxes
     take, :454-479) or with the FLOW_SMOOTHING_COMBINE debugger hook."""
     if cfg.TRACKING.LSTM_TEST.LSTM_TRACKING_ON:
         raise NotImplementedError('LSTM tracking is outside the device path')
+    _check_upper_bound_options(json_data, dets)
     if not cfg.TRACKING.FLOW_SMOOTHING_ON:
         return
     if cfg.TRACKING.DEBUG.FLOW_SMOOTHING_COMBINE:
@@ -401,7 +579,7 @@ def compute_matches_tracks(json_data, dets, lstm_model=None):
     """:669-708.  Splits images into videos by dirname, links every video in one
     batched device pass, writes dets['all_tracks'] = [[], per-image id lists].
     With TRACKING.FLOW_SMOOTHING_ON each video's poses and boxes are then smoothed along the flow (:695-697)."""
-    _check_tracking_options(dets)
+    _check_tracking_options(dets, json_data)
     num_imgs = len(json_data)
     all_tracks = [[]] * num_imgs
     all_video_roidb, video_entries = [], []
@@ -415,9 +593,12 @@ def compute_matches_tracks(json_data, dets, lstm_model=None):
         all_video_roidb.append(video_entries)
     assert num_imgs == sum(len(v) for v in all_video_roidb)
     logger.info('Computing tracks for %d videos.', len(all_video_roidb))
-    vids = [[_get_boxes(dets, det_id) for (_, det_id) in v] for v in all_video_roidb]
-    vposes = [[_get_poses(dets, det_id) for (_, det_id) in v] for v in all_video_roidb]
-    tracks = _tracks_for_videos(vids, vposes)
+    if cfg.TRACKING.DEBUG.UPPER_BOUND or cfg.TRACKING.DEBUG.UPPER_BOUND_5_GT_KPS_ONLY:
+        tracks = _upper_bound_tracks(all_video_roidb, dets)
+    else:
+        vids = [[_get_boxes(dets, det_id) for (_, det_id) in v] for v in all_video_roidb]
+        vposes = [[_get_poses(dets, det_id) for (_, det_id) in v] for v in all_video_roidb]
+        tracks = _tracks_for_videos(vids, vposes)
     if cfg.TRACKING.FLOW_SMOOTHING_ON:
         tracks = [_smooth_pose_video(entries, dets, tracks[v]) for v, entries in enumerate(all_video_roidb)]
     for v, entries in enumerate(all_video_roidb):
@@ -437,12 +618,14 @@ def run_posetrack_tracking(test_output_dir, json_data, write_json=True, dataset=
     if not osp.exists(det_file):
         raise ValueError('Output file not found {}'.format(det_file))
     logger.info('Tracking over %s', det_file)
+    if cfg.TRACKING.DEBUG.UPPER_BOUND_2_GT_KPS:        # :770-771
+        cfg.TRACKING.DEBUG.UPPER_BOUND = True
     dets = _load_det_file(det_file)
     if cfg.TRACKING.KEEP_CENTER_DETS_ONLY:
         _center_detections(dets)
     assert len(json_data) == len(dets['all_boxes'][1])
     assert len(json_data) == len(dets['all_keyps'][1])
-    _check_tracking_options(dets)
+    _check_tracking_options(dets, json_data)
     conf = cfg.TRACKING.CONF_FILTER_INITIAL_DETS
     logger.info('Pruning detections with less than %s confidence', conf)
     dets = _prune_bad_detections(dets, json_data, conf)

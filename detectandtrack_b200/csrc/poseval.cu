@@ -23,6 +23,34 @@ __device__ __forceinline__ double pt_pck(unsigned m, int ngtp) {
   return ngtp > 0 ? __ddiv_rn(c, (double)ngtp) : c;
 }
 
+// prToGT of a frame (:549-559) from the matched-joint masks [nP, nG] and the GT people's annotated joints: best_gt[p] =
+// np.argmax(pck, axis=1) (the first maximum), then pr2gt[g] = np.argmax of the pck pruned to those, -1 where it is 0.
+// Called by the whole CTA; ends synchronised.
+__device__ void pt_pr_to_gt(const uint16_t* mask, const uint16_t* gmask, int nP, int nG, int* best_gt, int* pr2gt) {
+  const int tid = threadIdx.x;
+  for (int p = tid; p < nP; p += blockDim.x) {
+    int best = 0;
+    double bv = pt_pck(mask[p * nG], __popc(gmask[0]));
+    for (int g = 1; g < nG; ++g) {
+      const double v = pt_pck(mask[p * nG + g], __popc(gmask[g]));
+      if (v > bv) { bv = v; best = g; }
+    }
+    best_gt[p] = best;
+  }
+  __syncthreads();
+  for (int g = tid; g < nG; g += blockDim.x) {
+    const int ng = __popc(gmask[g]);
+    int best = 0;
+    double bv = best_gt[0] == g ? pt_pck(mask[g], ng) : 0.0;
+    for (int p = 1; p < nP; ++p) {
+      const double v = best_gt[p] == g ? pt_pck(mask[p * nG + g], ng) : 0.0;
+      if (v > bv) { bv = v; best = p; }
+    }
+    pr2gt[g] = bv == 0.0 ? -1 : best;
+  }
+  __syncthreads();
+}
+
 __global__ void __launch_bounds__(256) pt_assign_kernel(const int* __restrict__ gt_off, const int* __restrict__ pr_off,
                                                         const long long* __restrict__ pair_off, int F,
                                                         const double* __restrict__ gt_rect, const double* __restrict__ gt_kp,
@@ -76,27 +104,8 @@ __global__ void __launch_bounds__(256) pt_assign_kernel(const int* __restrict__ 
     mask[e] = (uint16_t)m;
   }
   __syncthreads();
-  for (int p = tid; p < nP; p += blockDim.x) {                // np.argmax(pck, axis=1): the first maximum
-    int best = 0;
-    double bv = pt_pck(mask[p * nG], __popc(gmask[0]));
-    for (int g = 1; g < nG; ++g) {
-      const double v = pt_pck(mask[p * nG + g], __popc(gmask[g]));
-      if (v > bv) { bv = v; best = g; }
-    }
-    best_gt[p] = best;
-    assigned[p] = -1;
-  }
-  __syncthreads();
-  for (int g = tid; g < nG; g += blockDim.x) {                // np.argmax(pck, axis=0) of the pruned pck, -1 where 0
-    const int ng = __popc(gmask[g]);
-    int best = 0;
-    double bv = best_gt[0] == g ? pt_pck(mask[g], ng) : 0.0;
-    for (int p = 1; p < nP; ++p) {
-      const double v = best_gt[p] == g ? pt_pck(mask[p * nG + g], ng) : 0.0;
-      if (v > bv) { bv = v; best = p; }
-    }
-    pr2gt[g] = bv == 0.0 ? -1 : best;
-  }
+  pt_pr_to_gt(mask, gmask, nP, nG, best_gt, pr2gt);
+  for (int p = tid; p < nP; p += blockDim.x) assigned[p] = -1;
   __syncthreads();
   for (int g = tid; g < nG; g += blockDim.x)                  // a prediction is best for at most one GT (:597-598)
     if (pr2gt[g] >= 0) assigned[pr2gt[g]] = g;
@@ -311,6 +320,112 @@ __global__ void __launch_bounds__(1024) pt_rpc_kernel(const PtItem* __restrict__
   }
 }
 
+// ---- assignGTmulti(..., computeUpperBound=True) (:559-573) -------------------------------------------------------------
+
+// The frame's prToGT, recomputed from dt_posetrack_assign's dist (finite = the joint matched) into s_pr2gt; returns how
+// many predictions the upper-bound view keeps: those some GT selected, or all of them in a frame without both GT and
+// predictions (left untouched).
+__device__ int pt_ub_select(int f, const int* __restrict__ gt_off, const int* __restrict__ pr_off,
+                            const long long* __restrict__ pair_off, const double* __restrict__ gt_kp,
+                            const double* __restrict__ dist, uint16_t* mask, uint16_t* gmask, int* best_gt, int* s_pr2gt) {
+  const int tid = threadIdx.x;
+  const int g0 = gt_off[f], nG = gt_off[f + 1] - g0, nP = pr_off[f + 1] - pr_off[f];
+  if (nG == 0 || nP == 0) return nP;
+  for (int g = tid; g < nG; g += blockDim.x) {
+    unsigned m = 0;
+    for (int j = 0; j < PTJ; ++j) m |= (gt_kp[((size_t)(g0 + g) * PTJ + j) * 3 + 2] != 0.0) ? (1u << j) : 0u;
+    gmask[g] = (uint16_t)m;
+  }
+  const double* d = dist + (size_t)pair_off[f] * PTJ;
+  for (int e = tid; e < nP * nG; e += blockDim.x) {
+    unsigned m = 0;
+    for (int j = 0; j < PTJ; ++j) m |= isfinite(d[(size_t)e * PTJ + j]) ? (1u << j) : 0u;
+    mask[e] = (uint16_t)m;
+  }
+  __syncthreads();
+  pt_pr_to_gt(mask, gmask, nP, nG, best_gt, s_pr2gt);
+  int n = 0;
+  for (int g = 0; g < nG; ++g) n += s_pr2gt[g] >= 0;
+  return n;
+}
+
+// counts [nframes] of the view, written at ub_pr_off[f + 1]
+__global__ void __launch_bounds__(256) pt_ub_count_kernel(const int* __restrict__ gt_off, const int* __restrict__ pr_off,
+                                                          const long long* __restrict__ pair_off, const double* __restrict__ gt_kp,
+                                                          const double* __restrict__ dist, int* __restrict__ ub_pr_off) {
+  __shared__ uint16_t mask[DT_LSA_MAX_DIM * DT_PT_MAX_GT];
+  __shared__ uint16_t gmask[DT_PT_MAX_GT];
+  __shared__ int best_gt[DT_LSA_MAX_DIM];
+  __shared__ int pr2gt[DT_PT_MAX_GT];
+  const int n = pt_ub_select(blockIdx.x, gt_off, pr_off, pair_off, gt_kp, dist, mask, gmask, best_gt, pr2gt);
+  if (threadIdx.x == 0) ub_pr_off[blockIdx.x + 1] = n;
+}
+
+struct PtAddL { __device__ long long operator()(long long a, long long b) const { return a + b; } };
+
+// one CTA: ub_pr_off [F + 1] prefix-summed in place, ub_pair_off [F + 1] = prefix sums of nG * kept predictions
+__global__ void __launch_bounds__(1024) pt_ub_scan_kernel(const int* __restrict__ gt_off, int F, int* __restrict__ ub_pr_off,
+                                                          long long* __restrict__ ub_pair_off) {
+  __shared__ int shi[32];
+  __shared__ long long shl[32];
+  int carry = 0;
+  long long carry2 = 0;
+  for (int f0 = 0; f0 < F; f0 += blockDim.x) {
+    const int f = f0 + threadIdx.x;
+    const int c = f < F ? ub_pr_off[f + 1] : 0;
+    const long long pc = f < F ? (long long)c * (gt_off[f + 1] - gt_off[f]) : 0;
+    int t;
+    long long t2;
+    const int v = pt_block_scan(c, PtAdd(), shi, &t);
+    const long long v2 = pt_block_scan(pc, PtAddL(), shl, &t2);
+    if (f < F) { ub_pr_off[f + 1] = carry + v; ub_pair_off[f + 1] = carry2 + v2; }
+    carry += t;
+    carry2 += t2;
+  }
+  if (threadIdx.x == 0) { ub_pr_off[0] = 0; ub_pair_off[0] = 0; }
+}
+
+// one CTA per frame: the view's prediction rows (keypoints, track id) and distances
+__global__ void __launch_bounds__(256) pt_ub_gather_kernel(const int* __restrict__ gt_off, const int* __restrict__ pr_off,
+                                                           const long long* __restrict__ pair_off, const double* __restrict__ gt_kp,
+                                                           const int* __restrict__ gt_tid, const double* __restrict__ pr_kp,
+                                                           const int* __restrict__ pr_tid, const double* __restrict__ dist,
+                                                           const int* __restrict__ ub_pr_off,
+                                                           const long long* __restrict__ ub_pair_off, double* __restrict__ ub_pr_kp,
+                                                           int* __restrict__ ub_pr_tid, double* __restrict__ ub_dist) {
+  __shared__ uint16_t mask[DT_LSA_MAX_DIM * DT_PT_MAX_GT];
+  __shared__ uint16_t gmask[DT_PT_MAX_GT];
+  __shared__ int best_gt[DT_LSA_MAX_DIM];
+  __shared__ int pr2gt[DT_PT_MAX_GT];
+  __shared__ int sel_g[DT_PT_MAX_GT];                         // the k-th kept prediction's GT, in ascending GT order
+  const int f = blockIdx.x, tid = threadIdx.x;
+  const int g0 = gt_off[f], nG = gt_off[f + 1] - g0, p0 = pr_off[f], nP = pr_off[f + 1] - p0;
+  const int n = pt_ub_select(f, gt_off, pr_off, pair_off, gt_kp, dist, mask, gmask, best_gt, pr2gt);
+  const bool sel = nG > 0 && nP > 0;
+  if (sel && tid == 0) {
+    int k = 0;
+    for (int g = 0; g < nG; ++g) if (pr2gt[g] >= 0) sel_g[k++] = g;
+  }
+  __syncthreads();
+  const int o0 = ub_pr_off[f];
+  for (int e = tid; e < n * PTJ * 4; e += blockDim.x) {
+    const int k = e / (PTJ * 4), c = e - k * (PTJ * 4);
+    const int src = p0 + (sel ? pr2gt[sel_g[k]] : k);
+    ub_pr_kp[(size_t)(o0 + k) * PTJ * 4 + c] = pr_kp[(size_t)src * PTJ * 4 + c];
+  }
+  for (int k = tid; k < n; k += blockDim.x) {
+    const int src = p0 + (sel ? pr2gt[sel_g[k]] : k);
+    ub_pr_tid[o0 + k] = sel ? gt_tid[g0 + sel_g[k]] : pr_tid[src];        // trackidxPr = trackidxGT[sel_pos]
+  }
+  if (!sel) return;
+  const double* d = dist + (size_t)pair_off[f] * PTJ;
+  double* od = ub_dist + (size_t)ub_pair_off[f] * PTJ;
+  for (int e = tid; e < n * nG * PTJ; e += blockDim.x) {
+    const int k = e / (nG * PTJ), gj = e - k * (nG * PTJ);
+    od[e] = d[(size_t)pr2gt[sel_g[k]] * nG * PTJ + gj];
+  }
+}
+
 // ---- MOTAccumulator.update -------------------------------------------------------------------------------------------
 
 struct PtMotSmem {
@@ -507,6 +622,29 @@ extern "C" int dt_posetrack_assign(const int* gt_off, const int* pr_off, const l
                "dt_posetrack_assign: null pointer");
   pt_assign_kernel<<<nframes, 256, 0, (cudaStream_t)stream>>>(gt_off, pr_off, pair_off, nframes, gt_rect, gt_kp, pr_kp,
                                                               labels, ngt, dist);
+  DT_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int dt_posetrack_upper_bound(const int* gt_off, const int* pr_off, const long long* pair_off, int nframes,
+                                       const double* gt_kp, const int* gt_tid, const double* pr_kp, const int* pr_tid,
+                                       const double* dist, int max_gt, int max_pr, int* ub_pr_off, long long* ub_pair_off,
+                                       double* ub_pr_kp, int* ub_pr_tid, double* ub_dist, void* stream) {
+  DT_CHECK_ARG(nframes >= 0 && max_gt >= 0 && max_gt <= DT_PT_MAX_GT && max_pr >= 0 && max_pr <= DT_LSA_MAX_DIM,
+               "dt_posetrack_upper_bound: bad shape nframes=%d max_gt=%d max_pr=%d (max_gt <= %d, max_pr <= %d)", nframes,
+               max_gt, max_pr, DT_PT_MAX_GT, DT_LSA_MAX_DIM);
+  if (nframes == 0) return 0;
+  DT_CHECK_ARG(gt_off && pr_off && pair_off && ub_pr_off && ub_pair_off && (max_gt == 0 || (gt_kp && gt_tid)) &&
+               (max_pr == 0 || (pr_kp && pr_tid && ub_pr_kp && ub_pr_tid)) &&
+               (max_gt == 0 || max_pr == 0 || (dist && ub_dist)),
+               "dt_posetrack_upper_bound: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  pt_ub_count_kernel<<<nframes, 256, 0, st>>>(gt_off, pr_off, pair_off, gt_kp, dist, ub_pr_off);
+  DT_CHECK_LAUNCH();
+  pt_ub_scan_kernel<<<1, 1024, 0, st>>>(gt_off, nframes, ub_pr_off, ub_pair_off);
+  DT_CHECK_LAUNCH();
+  pt_ub_gather_kernel<<<nframes, 256, 0, st>>>(gt_off, pr_off, pair_off, gt_kp, gt_tid, pr_kp, pr_tid, dist, ub_pr_off,
+                                               ub_pair_off, ub_pr_kp, ub_pr_tid, ub_dist);
   DT_CHECK_LAUNCH();
   return 0;
 }

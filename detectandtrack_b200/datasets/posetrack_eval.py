@@ -2,6 +2,7 @@
 assignment, the per-joint AP and the CLEAR-MOT accumulation on the device (csrc/poseval.cu).
 
     evaluate(gtdir, preddir, eval_pose=True, eval_track=True, eval_upper_bound=False) -> ((apAll, preAll, recAll), metrics)
+    evaluate_upper_bound(gtdir, preddir, ...)       the same with poseval's upper-bound MOT (eval_helpers.py:559-573)
 
 The host part restates ``eval_helpers.load_data_dir`` + ``cleanupData`` + ``removeIgnoredPoints`` (eval_helpers.py:282-415)
 and packs the result into flat fp64 arrays (``PoseTrackPack``).  Everything after that (distances, PCK, the GT/prediction
@@ -333,8 +334,10 @@ def _map_capacity(pack, lists):
     return cap
 
 
-def evaluate_pack(pack, eval_pose=True, eval_track=True, per_video=False):
-    """The device evaluation of a loaded pack.  Returns {'ap': (apAll, preAll, recAll), 'metrics': metrics} and, with
+def evaluate_pack(pack, eval_pose=True, eval_track=True, per_video=False, track_upper_bound=False):
+    """The device evaluation of a loaded pack.  With track_upper_bound, the MOT counts (total and per video) come from
+    poseval's upper-bound view (assignGTmulti(..., computeUpperBound=True)): in every frame with both GT and predictions
+    only the predictions some GT selected are kept, with that GT's track id; AP is unchanged.  Returns {'ap': (apAll, preAll, recAll), 'metrics': metrics} and, with
     per_video, 'videos': {seq index: (ap, mota)} as evaluating each GT file alone gives them (NaN where that fails).
     'raw' holds the device outputs: labels [NP, 15], ngt [15, F], the segments' (AP, precision, recall) [nseg, 3] (the
     15 joints of all frames first when eval_pose, then 15 per sequence with per_video), and the MOT counts [L, 15, 4] /
@@ -376,7 +379,9 @@ def evaluate_pack(pack, eval_pose=True, eval_track=True, per_video=False):
     if lists:
         list_off = np.concatenate([[0], np.cumsum([len(x) for x in lists])]).astype(np.int64)
         frames = np.concatenate(lists).astype(np.int64)
-        counts, sumd, status = P.mot_counts(dp, dist, list_off, frames, _map_capacity(pack, lists))
+        mdp = P.upper_bound(dp, dist) if track_upper_bound else dp
+        counts, sumd, status = P.mot_counts(mdp, mdp.dist if track_upper_bound else dist, list_off, frames,
+                                            _map_capacity(pack, lists))
         torch.cuda.synchronize()
         if int(status.max()) != 0:
             raise RuntimeError('dt_posetrack_mot: a frame list exceeded its bounds')
@@ -451,15 +456,29 @@ def print_table(vals, motHeader=False):
 
 def evaluate(gtdir, preddir, eval_pose=True, eval_track=True, eval_upper_bound=False, per_video=False, verbose=True):
     """evaluate_simple.evaluate.  ((apAll, preAll, recAll) [16, 1], metrics [19, 1]), NaN where not evaluated; with
-    per_video also {GT file name: (ap, mota)} as a third element."""
+    per_video also {GT file name: (ap, mota)} as a third element.
+
+    eval_upper_bound raises NotImplementedError: the upper bound replaces the predictions' track ids with the GT's, so a
+    call that asks for it names it explicitly through evaluate_upper_bound(), and a MOTA from evaluate() is always the
+    predictions' own."""
     if eval_upper_bound:
-        raise NotImplementedError('TRACKING.DEBUG.UPPER_BOUND_4_EVAL_UPPER_BOUND (the upper-bound tracking evaluation) '
-                                  'is not implemented')
+        raise NotImplementedError('evaluate() scores the predictions as they are; the upper-bound tracking evaluation '
+                                  '(TRACKING.DEBUG.UPPER_BOUND_4_EVAL_UPPER_BOUND) is evaluate_upper_bound()')
+    return _evaluate(gtdir, preddir, eval_pose, eval_track, False, per_video, verbose)
+
+
+def evaluate_upper_bound(gtdir, preddir, eval_pose=True, eval_track=True, per_video=False, verbose=True):
+    """evaluate_simple.evaluate(..., eval_upper_bound=True): as evaluate(), with the MOT metrics of poseval's upper bound
+    (every prediction a GT selected takes that GT's track id, the others are dropped from the MOT inputs)."""
+    return _evaluate(gtdir, preddir, eval_pose, eval_track, True, per_video, verbose)
+
+
+def _evaluate(gtdir, preddir, eval_pose, eval_track, track_upper_bound, per_video, verbose):
     gtFramesAll, prFramesAll, names = load_data_dir(gtdir, preddir)
     if verbose:
         print('# gt frames  :', len(gtFramesAll))
         print('# pred frames:', len(prFramesAll))
-    res = evaluate_pack(PoseTrackPack(gtFramesAll, prFramesAll, names), eval_pose, eval_track, per_video)
+    res = evaluate_pack(PoseTrackPack(gtFramesAll, prFramesAll, names), eval_pose, eval_track, per_video, track_upper_bound)
     if verbose and eval_pose:
         print('Average Precision (AP) metric:')
         print_table(res['ap'][0])

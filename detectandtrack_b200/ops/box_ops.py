@@ -189,3 +189,52 @@ def prune_detections(boxes, counts, hw, conf, T=1, center_only=True, min_area=50
     L.call('dt_prune_detections', L.ptr(boxes), F, dmax, ld, T, int(bool(center_only)), L.ptr(counts), L.ptr(hw),
            float(conf), float(min_area), L.ptr(out), L.ptr(counts_out), L.ptr(sel), L.stream_ptr())
     return out, counts_out, sel
+
+
+def gt_frame_costs(boxes, counts, poses=None, T=1, w_iou=1.0, w_pck=0.0, head_top=2, head_bottom=1, dist_thresh=0.5):
+    """boxes [2F, Dmax, ld], poses [2F, Dmax, R, K] (or None): the GT of frame f at entry 2f, its detections at 2f + 1 ->
+    cost [F, Dmax, Dmax] fp32, rows = GT (tracking_engine.py:287-296 with the frame's GT as the previous frame)."""
+    torch = L.require_cuda()
+    boxes = _f32c(boxes, torch)
+    F2, dmax, ld = boxes.shape
+    counts = counts.to(device='cuda', dtype=torch.int32).contiguous()
+    R = K = 0
+    if poses is not None:
+        poses = _f32c(poses, torch)
+        R, K = poses.shape[2], poses.shape[3]
+    cost = torch.empty((F2 // 2, dmax, dmax), dtype=torch.float32, device='cuda')
+    L.call('dt_gt_frame_costs', L.ptr(boxes), ld, T, L.ptr(poses), R, K, int(head_top), int(head_bottom), float(dist_thresh),
+           L.ptr(counts), F2 // 2, dmax, float(w_iou), float(w_pck), L.ptr(cost), L.stream_ptr())
+    return cost
+
+
+def _rows_arg(m, F, dmax):
+    """An int32 matches tensor as (pointer, row stride): [F, ld] as it is, or the detection rows of an interleaved [2F, dmax]."""
+    if m is None:
+        return None, 0
+    assert m.dtype.is_floating_point is False and m.is_contiguous()
+    if m.shape[0] == 2 * F:
+        return C.c_void_p(m.data_ptr() + dmax * m.element_size()), 2 * m.shape[1]
+    assert m.shape[0] == F
+    return L.ptr(m), m.shape[1]
+
+
+def track_upper_bound(boxes, poses, counts, gt_tid, matches=None, matches_gt=None, flags=0):
+    """TRACKING.DEBUG.UPPER_BOUND* on the interleaved packing of gt_frame_costs: boxes [2F, Dmax, ld], poses [2F, Dmax, R, K],
+    counts [2F], gt_tid [F, Dmax]; matches / matches_gt [F, ld] or the interleaved [2F, Dmax] output of match_frames.
+    Returns (boxes [F, Dmax, ld], poses [F, Dmax, R, K], track ids [F, Dmax], counts [F])."""
+    torch = L.require_cuda()
+    boxes, poses = _f32c(boxes, torch), _f32c(poses, torch)
+    F2, dmax, ld = boxes.shape
+    F, R, K = F2 // 2, poses.shape[2], poses.shape[3]
+    counts = counts.to(device='cuda', dtype=torch.int32).contiguous()
+    gt_tid = gt_tid.to(device='cuda', dtype=torch.int32).contiguous()
+    out_b = torch.empty((F, dmax, ld), dtype=torch.float32, device='cuda')
+    out_p = torch.empty((F, dmax, R, K), dtype=torch.float32, device='cuda')
+    out_t = torch.empty((F, dmax), dtype=torch.int32, device='cuda')
+    out_n = torch.empty((F,), dtype=torch.int32, device='cuda')
+    m, ldm = _rows_arg(matches, F, dmax)
+    mg, ldmg = _rows_arg(matches_gt, F, dmax)
+    L.call('dt_track_upper_bound', L.ptr(boxes), ld, L.ptr(poses), R, K, L.ptr(counts), L.ptr(gt_tid), F, dmax, m, ldm, mg, ldmg,
+           int(flags), L.ptr(out_b), L.ptr(out_p), L.ptr(out_t), L.ptr(out_n), L.stream_ptr())
+    return out_b, out_p, out_t, out_n

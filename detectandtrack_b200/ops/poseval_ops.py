@@ -74,3 +74,21 @@ def mot_counts(dp, dist, list_off, list_frames, map_cap):
            L.ptr(dp.pr_kp), L.ptr(dp.pr_tid), L.ptr(dist), L.ptr(d_off), L.ptr(d_frames), nl, dp.max_gt, dp.max_pr,
            int(map_cap), L.ptr(counts), L.ptr(sumd), L.ptr(status), L.stream_ptr())
     return counts, sumd, status
+
+
+def upper_bound(dp, dist):
+    """The upper-bound view of the predictions (assignGTmulti with computeUpperBound) -> a DevicePack-like object whose
+    pr_off / pair_off / pr_kp / pr_tid are the view's, plus dist (its distances)."""
+    torch = L.require_cuda()
+    n = max(dp.pr_kp.shape[0], 1)
+    v = DevicePack.__new__(DevicePack)
+    v.__dict__.update(dp.__dict__)
+    v.pr_off = torch.empty((dp.F + 1,), dtype=torch.int32, device='cuda')
+    v.pair_off = torch.empty((dp.F + 1,), dtype=torch.int64, device='cuda')
+    v.pr_kp = torch.zeros((n, L.PT_JOINTS, 4), dtype=torch.float64, device='cuda')
+    v.pr_tid = torch.full((n,), -1, dtype=torch.int32, device='cuda')
+    v.dist = torch.empty_like(dist)
+    L.call('dt_posetrack_upper_bound', L.ptr(dp.gt_off), L.ptr(dp.pr_off), L.ptr(dp.pair_off), dp.F, L.ptr(dp.gt_kp),
+           L.ptr(dp.gt_tid), L.ptr(dp.pr_kp), L.ptr(dp.pr_tid), L.ptr(dist), dp.max_gt, dp.max_pr, L.ptr(v.pr_off),
+           L.ptr(v.pair_off), L.ptr(v.pr_kp), L.ptr(v.pr_tid), L.ptr(v.dist), L.stream_ptr())
+    return v

@@ -132,6 +132,28 @@ int dt_frame_costs(const float* boxes, int ldb, int T, const float* poses, int l
                    float dist_thresh, const int* counts, const unsigned char* is_start, int nframes, int dmax, float w_iou,
                    double w_pck, float* cost, void* stream);
 
+/* ---- upper_bound.cu: TRACKING.DEBUG.UPPER_BOUND* (lib/core/tracking_engine.py:272-350) ---- */
+#define DT_UB_COMPACT 1     /* UPPER_BOUND: keep the detections a GT took, with the GT's track id */
+#define DT_UB_GT_KPS 2      /* UPPER_BOUND_2_GT_KPS: the GT's box and keypoint rows 0..2 on every kept detection */
+#define DT_UB_ONLY_CONF 4   /* UPPER_BOUND_2_GT_KPS_ONLY_CONF: keypoint row 2 only */
+
+/* GT-vs-detection cost matrices of every frame: boxes [2 * nframes, dmax, ld] and poses [2 * nframes, dmax, R, K] hold the
+ * GT of frame f at entry 2f (boxes padded with a score column, integer-valued keypoints in rows 0..2) and its detections at
+ * entry 2f + 1; counts [2 * nframes].  cost [nframes, dmax, dmax] fp32, rows = GT, = fp32(fp32(w_iou * (1 - IoU)) + w_pck *
+ * pck) with the pck term in fp64 (numpy promotes the reference's int32 GT keypoints so); 0 beyond the counts.  Feed to
+ * dt_lsa_batched with nrows = counts[2f], ncols = counts[2f + 1]. */
+int dt_gt_frame_costs(const float* boxes, int ld, int T, const float* poses, int R, int K, int head_top, int head_bottom,
+                      double dist_thresh, const int* counts, int nframes, int dmax, float w_iou, double w_pck, float* cost,
+                      void* stream);
+/* One CTA per frame of the same packing: matches [nframes, ldm] (detection -> GT row or -1, the configured cost; needed
+ * with DT_UB_COMPACT) and matches_gt [nframes, ldmg] (the bbox Hungarian match of UPPER_BOUND_5_GT_KPS_ONLY, may be NULL).
+ * gt_tid [nframes, dmax].  Outputs, rows compacted in ascending detection order under DT_UB_COMPACT: out_boxes [nframes,
+ * dmax, ld], out_poses [nframes, dmax, R, K] (matches_gt's GT rows 0..2 win over DT_UB_GT_KPS's, as in the reference),
+ * out_tid [nframes, dmax] (the GT track id, -1 without DT_UB_COMPACT), out_counts [nframes]. */
+int dt_track_upper_bound(const float* boxes, int ld, const float* poses, int R, int K, const int* counts, const int* gt_tid,
+                         int nframes, int dmax, const int* matches, int ldm, const int* matches_gt, int ldmg, int flags,
+                         float* out_boxes, float* out_poses, int* out_tid, int* out_counts, void* stream);
+
 /* lib/core/tracking_engine.py:272-350 id propagation.  video_first [nvideos]
  * (device) = index of the first frame of each video, ascending.  tracks
  * [nframes, dmax] (-1 beyond counts[f]).  ids: next_id++, and
@@ -626,6 +648,15 @@ int dt_flow_smooth_poses(const float* poses, const float* boxes, const int* coun
 int dt_posetrack_assign(const int* gt_off, const int* pr_off, const long long* pair_off, int nframes, const double* gt_rect,
                         const double* gt_kp, const double* pr_kp, int max_gt, int max_pr, signed char* labels, int* ngt,
                         double* dist, void* stream);
+/* The upper-bound view of the predictions (assignGTmulti with computeUpperBound, eval_helpers.py:559-573) for
+ * dt_posetrack_mot: in a frame with both GT and predictions only the predictions some GT selected (prToGT, recomputed from
+ * dist) are kept, in ascending GT order, with that GT's track id; other frames are copied.  Outputs: ub_pr_off [nframes + 1],
+ * ub_pair_off [nframes + 1], ub_pr_kp [NP, 15, 4], ub_pr_tid [NP] and ub_dist [pair_off[nframes], 15], each filled up to
+ * the view's own totals. */
+int dt_posetrack_upper_bound(const int* gt_off, const int* pr_off, const long long* pair_off, int nframes, const double* gt_kp,
+                             const int* gt_tid, const double* pr_kp, const int* pr_tid, const double* dist, int max_gt, int max_pr,
+                             int* ub_pr_off, long long* ub_pair_off, double* ub_pr_kp, int* ub_pr_tid, double* ub_dist,
+                             void* stream);
 /* Workspace of dt_posetrack_ap for nentries scores in all. */
 int dt_posetrack_ap_workspace_bytes(long long nentries, size_t* bytes /*host out*/);
 /* evaluateAP.computeMetrics (computeRPC + VOCap) of every segment: segs [nseg, 3] = (joint, first frame, end frame),
