@@ -102,6 +102,9 @@ HOST_FUNCS = {'dt_planes_ld': ([_i, _i, _i, _i], C.c_int), 'dt_jpeg_available': 
               'dt_posetrack_mot_smem_bytes': ([_i, _i, _i, C.POINTER(_sz)], C.c_int),
               'dt_posetrack_mot': ([_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _p], C.c_int),
               'dt_posetrack_upper_bound': ([_p, _p, _p, _i, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p], C.c_int),
+              # the fp64 solver of the pose-pck tracking cost: a launcher too, with its argument-error cases in
+              # tests/test_capi_errors.py::test_lsa_batched_f64_argument_checks
+              'dt_lsa_batched_f64': ([_p, _i, _i, _i, _p, _p, _i, _p, _p, _p], C.c_int),
               # TRACKING.DEBUG.UPPER_BOUND* kernels: launchers too, with their argument-error cases in tests/test_upper_bound.py
               'dt_gt_frame_costs': ([_p, _i, _i, _p, _i, _i, _i, _i, C.c_double, _p, _i, _i, _f, C.c_double, _p, _p], C.c_int),
               'dt_track_upper_bound': ([_p, _i, _p, _i, _i, _p, _p, _i, _i, _p, _i, _p, _i, _i, _p, _p, _p, _p, _p], C.c_int)}

@@ -186,14 +186,14 @@ def _compute_matches(prev_frame_data, cur_frame_data, prev_boxes, cur_boxes,
     if bipart_match_algo not in box_ops.ALGOS:
         raise NotImplementedError('Unknown matching algo: {}'.format(bipart_match_algo))
     if C is not None:
-        C = np.ascontiguousarray(C, dtype=np.float32)
+        # scipy solves the matrix in fp64: a float32 one is exact in fp32, any other is solved in fp64
+        C = np.ascontiguousarray(C, dtype=np.float32 if np.asarray(C).dtype == np.float32 else np.float64)
         P, Q = C.shape
         if P == 0 or Q == 0:
             return -np.ones((Q,), dtype=np.int32)
         m, status = box_ops.lsa_batched(torch.from_numpy(C).cuda().unsqueeze(0),
                                         torch.tensor([P]), torch.tensor([Q]), bipart_match_algo)
-        if int(status[0].item()) != 0:
-            raise ValueError('cost matrix is infeasible')
+        _check_status(status)
         return m[0, :Q].cpu().numpy().astype(np.int32)
     weight = _check_default_cost(cost_types, cost_weights)
     nboxes = cur_boxes.shape[0]
@@ -204,6 +204,13 @@ def _compute_matches(prev_frame_data, cur_frame_data, prev_boxes, cur_boxes,
     m, _ = box_ops.match_frames(torch.from_numpy(packed).cuda(), torch.from_numpy(counts), None, T=T, weight=weight,
                                 algo=bipart_match_algo)
     return m[1, :nboxes].cpu().numpy().astype(np.int32)
+
+
+def _check_status(*statuses):
+    """scipy's ValueError for a cost matrix it cannot solve: the solver's status 1 (infeasible, or a NaN / -inf entry)."""
+    for st in statuses:
+        if st is not None and bool(st.cpu().numpy().any()):
+            raise ValueError('cost matrix is infeasible or contains invalid numeric entries')
 
 
 def _pose_cost_args(videos_poses, kpt_names=None):
@@ -237,9 +244,9 @@ def _tracks_for_videos(videos_boxes, videos_poses=None, kpt_names=None, videos_p
     d_counts = torch.from_numpy(counts).cuda()
     d_start = torch.from_numpy(is_start).cuda()
     if w_pck == 0.0:
-        matches, _ = box_ops.match_frames(torch.from_numpy(packed).cuda(), d_counts, d_start, T=T, weight=w_iou, algo=algo)
+        matches, status = box_ops.match_frames(torch.from_numpy(packed).cuda(), d_counts, d_start, T=T, weight=w_iou, algo=algo)
     elif videos_prev_poses is not None:
-        matches = _pair_matches(flat, first, videos_poses, videos_prev_poses, packed.shape[1], w_iou, w_pck, algo, kpt_names)
+        matches, status = _pair_matches(flat, first, videos_poses, videos_prev_poses, packed.shape[1], w_iou, w_pck, algo, kpt_names)
     else:
         # combined cost (tracking_engine.py:158-181): cost matrices of every frame pair in one launch, then the batched solver
         assert videos_poses is not None, "the 'pose-pck' cost needs the poses of every detection"
@@ -251,6 +258,7 @@ def _tracks_for_videos(videos_boxes, videos_poses=None, kpt_names=None, videos_p
         matches, status = box_ops.lsa_batched(cost, nrows, d_counts, algo)
     tracks = box_ops.assign_track_ids(matches, d_counts, torch.tensor(first, dtype=torch.int32), d_start)
     tracks = tracks.cpu().numpy()
+    _check_status(status)
     out = []
     for v, vb in enumerate(videos_boxes):
         f0 = first[v]
@@ -261,7 +269,8 @@ def _tracks_for_videos(videos_boxes, videos_poses=None, kpt_names=None, videos_p
 def _pair_matches(flat, first, videos_poses, videos_prev_poses, dmax, w_iou, w_pck, algo, kpt_names=None):
     """The combined cost of every frame pair (f - 1, f) of every video with frame f - 1's poses taken from
     videos_prev_poses: the pairs are packed pair-interleaved, [(f - 1, f), ...] with is_start on every first entry, for
-    dt_frame_costs + dt_lsa_batched.  Returns matches [F, dmax] in frame order (first frames of videos: -1)."""
+    dt_frame_costs + dt_lsa_batched_f64.  Returns matches [F, dmax] in frame order (first frames of videos: -1) and the
+    solver's status per pair (None without pairs)."""
     import torch
     F = len(flat)
     cur = [p for vp in videos_poses for p in vp]
@@ -271,7 +280,7 @@ def _pair_matches(flat, first, videos_poses, videos_prev_poses, dmax, w_iou, w_p
     pair_of = [f for f in range(F) if not is_first[f]]
     out = torch.full((F, dmax), -1, dtype=torch.int32, device='cuda')
     if not pair_of:
-        return out
+        return out, None
     boxes, pposes = [], []
     for f in pair_of:
         boxes += [flat[f - 1], flat[f]]
@@ -286,10 +295,10 @@ def _pair_matches(flat, first, videos_poses, videos_prev_poses, dmax, w_iou, w_p
     cost = box_ops.frame_costs(torch.from_numpy(packed).cuda(), d_counts, torch.from_numpy(is_start).cuda(),
                                torch.from_numpy(poses).cuda(), T=T, w_iou=w_iou, w_pck=w_pck, head_top=ht, head_bottom=hb)
     nrows = torch.cat([d_counts[:1] * 0, d_counts[:-1]]) * (1 - torch.from_numpy(is_start).cuda().to(torch.int32))
-    m, _ = box_ops.lsa_batched(cost, nrows, d_counts, algo)
+    m, status = box_ops.lsa_batched(cost, nrows, d_counts, algo)
     w = min(dmax, m.shape[1])
     out[torch.tensor(pair_of, device='cuda'), :w] = m[1::2, :w]
-    return out
+    return out, status
 
 
 # ------------------------------------------------------------------------------ upper-bound experiments
@@ -389,16 +398,17 @@ def _upper_bound_tracks(all_video_roidb, dets):
     is_start[0::2] = 1
     d_b, d_p, d_n = torch.from_numpy(pb).cuda(), torch.from_numpy(pp).cuda(), torch.from_numpy(cnt).cuda()
     d_s = torch.from_numpy(is_start).cuda()
-    matches = matches_gt = None
+    matches = matches_gt = status = status_gt = None
     if ub:
         if w_pck == 0.0:
-            matches, _ = box_ops.match_frames(d_b, d_n, d_s, T=T, weight=w_iou, algo=algo)
+            matches, status = box_ops.match_frames(d_b, d_n, d_s, T=T, weight=w_iou, algo=algo)
         else:
             _, ht, hb = _pose_cost_args([poses])
             cost = box_ops.gt_frame_costs(d_b, d_n, d_p, T=T, w_iou=w_iou, w_pck=w_pck, head_top=ht, head_bottom=hb)
-            matches, _ = box_ops.lsa_batched(cost, d_n[0::2], d_n[1::2], algo)
+            matches, status = box_ops.lsa_batched(cost, d_n[0::2], d_n[1::2], algo)
     if ub5:                                                   # bbox-overlap, weight 1, hungarian (:329-333)
-        matches_gt, _ = box_ops.match_frames(d_b, d_n, d_s, T=T, weight=1.0, algo='hungarian')
+        matches_gt, status_gt = box_ops.match_frames(d_b, d_n, d_s, T=T, weight=1.0, algo='hungarian')
+    _check_status(status, status_gt)
     flags = (box_ops.L.UB_COMPACT if ub else 0) | (box_ops.L.UB_GT_KPS if ub and ub2 else 0) | \
         (box_ops.L.UB_ONLY_CONF if ub and ub2 and conf_only else 0)
     ob, op, ot, on = box_ops.track_upper_bound(d_b, d_p, d_n, torch.from_numpy(tid).cuda(), matches, matches_gt, flags)

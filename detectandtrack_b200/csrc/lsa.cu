@@ -27,7 +27,7 @@ __device__ __forceinline__ float iou_pair_ref_l(const float* __restrict__ b, con
   return __fdiv_rn(inter, ua);
 }
 
-// The tracker's cost matrices are float32 and sized for dmax x dmax.
+// The bbox-only cost matrices are float32 (as the reference's) and staged in shared memory, dmax x dmax.
 using LsaSmem = LsaSmemT<float>;
 
 __host__ __device__ inline size_t lsa_smem_bytes(int dmax) { return lsa_smem_bytes_t<float>(dmax, (size_t)dmax * dmax); }
@@ -40,8 +40,10 @@ __device__ __forceinline__ LsaSmem lsa_carve(unsigned char* base, int dmax) {
 // mode 1: frames given [F, dmax, ld] boxes (+score col ignored); problem f = (frame f-1, frame f)
 // bipartite_matching_greedy (tracking_engine.py:184-206): repeatedly take the global argmin of the
 // remaining matrix (np.argmin: first occurrence in row-major order; deleting rows / columns keeps that
-// order, so ties go to the lowest remaining (row, col)).  s.C holds cost[p*Q + q]; SR / SC mark used rows / cols.
-__device__ void greedy_match_warp(const LsaSmem& s, int P, int Q, int* __restrict__ out) {
+// order, so ties go to the lowest remaining (row, col)).  C[p * ld + q] holds cost(p, q) (shared or global memory);
+// s.SR / s.SC mark used rows / cols.
+template <typename T>
+__device__ void greedy_match_warp(const LsaSmemT<T>& s, const T* C, int ld, int P, int Q, int* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const unsigned FULL = 0xffffffffu;
   for (int x = lane; x < P; x += 32) s.SR[x] = 0;
@@ -49,18 +51,18 @@ __device__ void greedy_match_warp(const LsaSmem& s, int P, int Q, int* __restric
   __syncwarp();
   const int steps = min(P, Q);
   for (int k = 0; k < steps; ++k) {
-    float bv = CUDART_INF_F; int bi = 0x7fffffff;
+    T bv = (T)CUDART_INF; int bi = 0x7fffffff;
     bool any = false;
     for (int e = lane; e < P * Q; e += 32) {
       const int p = e / Q, q = e - p * Q;
       if (s.SR[p] || s.SC[q]) continue;
-      const float c = s.C[e];
+      const T c = C[(size_t)p * ld + q];
       if (!any || c < bv) { bv = c; bi = e; any = true; }          // strict '<': first occurrence per lane
     }
     if (!any) bi = 0x7fffffff;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(FULL, bv, o);
+      const T ov = __shfl_xor_sync(FULL, bv, o);
       const int oi = __shfl_xor_sync(FULL, bi, o);
       const bool take = (oi != 0x7fffffff) && (bi == 0x7fffffff || ov < bv || (ov == bv && oi < bi));
       if (take) { bv = ov; bi = oi; }
@@ -99,11 +101,13 @@ __global__ void lsa_kernel(int mode, int algo, const float* __restrict__ src, in
   const bool transpose = (algo == 0) && Q < P;       // scipy: "tall matrix must be transposed"
   const int nr = transpose ? Q : P, nc = transpose ? P : Q;
   // stage the internal matrix: internal(i, j) = cost(prev = transpose ? j : i, cur = transpose ? i : j)
+  bool invalid = false;
   for (int e = lane; e < P * Q; e += 32) {
     const int p = e / Q, q = e - p * Q;              // coalesced over q in the source
     float c;
     if (mode == 0) {
       c = Cg[(size_t)p * ld + q];
+      invalid |= (c != c) || c == -CUDART_INF_F;     // scipy: "matrix contains invalid numeric entries"
     } else {
       const float* pb = prev + (size_t)p * ld;
       const float* qb = cur + (size_t)q * ld;
@@ -115,11 +119,45 @@ __global__ void lsa_kernel(int mode, int algo, const float* __restrict__ src, in
     if (transpose) s.C[(size_t)q * nc + p] = c; else s.C[(size_t)p * nc + q] = c;
   }
   __syncwarp();
-  if (algo == 1) { greedy_match_warp(s, P, Q, out); return; }
+  if (algo == 1) { greedy_match_warp(s, s.C, Q, P, Q, out); return; }
+  if (mode == 0 && __any_sync(0xffffffffu, invalid)) { if (lane == 0 && status) status[b] = 1; return; }
   const bool ok = lsa_solve_warp(s, nr, nc);
   if (!ok) { if (lane == 0 && status) status[b] = 1; return; }
   __syncwarp();
   // matches[cur] = prev (tracking_engine.py:244-246)
+  for (int i = lane; i < nr; i += 32) {
+    const int j = s.col4row[i];
+    if (transpose) out[i] = j; else out[j] = i;
+  }
+}
+
+// The same assignment on fp64 costs [B, dmax, ldc] (the combined pose-pck cost: the reference's matrix is float64 then).
+// An fp64 224 x 224 matrix does not fit in shared memory, so the solver reads it where it lies (one problem is at most
+// 400 KB, which stays in L2 while the warp walks it); a problem with Q < P is solved on the transpose by strided reads.
+__global__ void lsa_f64_kernel(int algo, const double* __restrict__ cost, int dmax, int ldc, const int* __restrict__ nrows,
+                               const int* __restrict__ ncols, int* __restrict__ matches, int* __restrict__ status) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int b = blockIdx.x, lane = threadIdx.x;
+  const LsaSmemT<double> s = lsa_carve_t<double>(smem_raw, dmax, 0);
+  const int P = min(max(nrows[b], 0), dmax), Q = min(max(ncols[b], 0), dmax);
+  const double* Cg = cost + (size_t)b * dmax * ldc;
+  int* out = matches + (size_t)b * dmax;
+  for (int q = lane; q < dmax; q += 32) out[q] = -1;
+  if (lane == 0 && status) status[b] = 0;
+  if (P == 0 || Q == 0) return;
+  if (algo == 1) { greedy_match_warp(s, Cg, ldc, P, Q, out); return; }
+  bool invalid = false;
+  for (int e = lane; e < P * Q; e += 32) {
+    const int p = e / Q, q = e - p * Q;
+    const double c = Cg[(size_t)p * ldc + q];
+    invalid |= (c != c) || c == -CUDART_INF;
+  }
+  if (__any_sync(0xffffffffu, invalid)) { if (lane == 0 && status) status[b] = 1; return; }
+  const bool transpose = Q < P;
+  const int nr = transpose ? Q : P, nc = transpose ? P : Q;
+  const LsaRows<double> rows{Cg, transpose ? (size_t)1 : (size_t)ldc, transpose ? (size_t)ldc : (size_t)1};
+  if (!lsa_solve_warp_rows(s, rows, nr, nc)) { if (lane == 0 && status) status[b] = 1; return; }
+  __syncwarp();
   for (int i = lane; i < nr; i += 32) {
     const int j = s.col4row[i];
     if (transpose) out[i] = j; else out[j] = i;
@@ -151,20 +189,19 @@ __global__ void pose_pck_kernel(const float* __restrict__ a, int P, const float*
 }
 
 // Cost matrices of all frame pairs of a batch of videos (tracking_engine.py:158-181): cost[f][p][q] (p = detection of frame
-// f-1, q = detection of frame f) = fp32( w_iou * (1 - IoU) [float32, as the reference computes it] + w_pck * pck [fp64] ),
-// summed in fp64 like np.sum(np.stack(all_Cs)); first frames of videos and entries beyond the counts are 0.
+// f-1, q = detection of frame f) = w_iou * (1 - IoU) [float32, as the reference computes it] + w_pck * pck [fp64], summed
+// and kept in fp64 like np.sum(np.stack(all_Cs)); first frames of videos and entries beyond the counts are 0.
 __global__ void frame_costs_kernel(const float* __restrict__ boxes, int ldb, int T, const float* __restrict__ poses, int ldp, int K,
                                    int ht, int hb, float thr, const int* __restrict__ counts, const unsigned char* __restrict__ is_start,
-                                   int dmax, float w_iou, double w_pck, float* __restrict__ cost) {
+                                   int dmax, float w_iou, double w_pck, double* __restrict__ cost) {
   const int f = blockIdx.x;
-  float* C = cost + (size_t)f * dmax * dmax;
+  double* C = cost + (size_t)f * dmax * dmax;
   const bool start = (f == 0) || (is_start && is_start[f]);
   const int P = start ? 0 : min(counts[f - 1], dmax), Q = min(counts[f], dmax);
   for (int e = threadIdx.x; e < dmax * dmax; e += blockDim.x) {
     const int p = e / dmax, q = e - p * dmax;
-    float c = 0.f;
+    double acc = 0.0;
     if (p < P && q < Q) {
-      double acc = 0.0;
       if (w_iou != 0.f) {
         const float* pb = boxes + ((size_t)(f - 1) * dmax + p) * ldb;
         const float* qb = boxes + ((size_t)f * dmax + q) * ldb;
@@ -174,9 +211,8 @@ __global__ void frame_costs_kernel(const float* __restrict__ boxes, int ldb, int
       }
       if (w_pck != 0.0)
         acc = __dadd_rn(acc, __dmul_rn(pck_cost(poses + ((size_t)(f - 1) * dmax + p) * ldp, poses + ((size_t)f * dmax + q) * ldp, K, ht, hb, thr), w_pck));
-      c = __double2float_rn(acc);
     }
-    C[e] = c;
+    C[e] = acc;
   }
 }
 
@@ -288,6 +324,19 @@ extern "C" int dt_lsa_batched(const float* cost, int batch, int dmax, int ldc, c
   return lsa_launch(0, algo, cost, batch, dmax, ldc, 1, nrows, ncols, nullptr, 1.f, matches, status, (cudaStream_t)stream);
 }
 
+extern "C" int dt_lsa_batched_f64(const double* cost, int batch, int dmax, int ldc, const int* nrows,
+                                  const int* ncols, int algo, int* matches, int* status, void* stream) {
+  DT_CHECK_ARG(algo == DT_MATCH_HUNGARIAN || algo == DT_MATCH_GREEDY, "dt_lsa_batched_f64: unknown algo %d", algo);
+  DT_CHECK_ARG(batch >= 0 && dmax >= 1 && dmax <= DT_LSA_MAX_DIM && ldc >= dmax,
+               "dt_lsa_batched_f64: bad shape batch=%d dmax=%d ldc=%d (dmax <= %d, ldc >= dmax)", batch, dmax, ldc, DT_LSA_MAX_DIM);
+  if (batch == 0) return 0;
+  DT_CHECK_ARG(cost && nrows && ncols && matches, "dt_lsa_batched_f64: null pointer");
+  const size_t smem = lsa_smem_bytes_t<double>(dmax, 0);
+  lsa_f64_kernel<<<batch, 32, smem, (cudaStream_t)stream>>>(algo, cost, dmax, ldc, nrows, ncols, matches, status);
+  DT_CHECK_LAUNCH();
+  return 0;
+}
+
 extern "C" int dt_match_frames(const float* frames, int nframes, int dmax, int ld, int T,
                                const int* counts, const unsigned char* is_start, float weight, int algo,
                                int* matches, int* status, void* stream) {
@@ -338,7 +387,7 @@ extern "C" int dt_pose_pck_cost(const float* a, int P, const float* b, int Q, in
 
 extern "C" int dt_frame_costs(const float* boxes, int ldb, int T, const float* poses, int ldp, int K, int head_top, int head_bottom,
                               float dist_thresh, const int* counts, const unsigned char* is_start, int nframes, int dmax,
-                              float w_iou, double w_pck, float* cost, void* stream) {
+                              float w_iou, double w_pck, double* cost, void* stream) {
   DT_CHECK_ARG(nframes >= 0 && dmax >= 1 && T >= 1 && T <= DT_MAX_T && ldb >= 4 * T, "dt_frame_costs: bad shape nframes=%d dmax=%d T=%d ldb=%d", nframes, dmax, T, ldb);
   DT_CHECK_ARG(w_pck == 0.0 || (poses && K >= 1 && ldp >= 2 * K && head_top >= 0 && head_top < K && head_bottom >= 0 && head_bottom < K),
                "dt_frame_costs: the pose-pck term needs poses [nframes, dmax, ldp >= 2K] and valid head joint indices");

@@ -1,6 +1,7 @@
 // Warp-parallel rectangular min-cost assignment in scipy.optimize.linear_sum_assignment's own visiting order, shared by
-// the tracker (lsa.cu, fp32 costs as the reference's cost matrices are float32) and the PoseTrack CLEAR-MOT accumulator
-// (poseval.cu, fp64 costs as py-motmetrics hands scipy the fp64 distances).
+// the tracker (lsa.cu: the bbox-only cost in fp32 from shared memory, as the reference's matrix is float32; the combined
+// pose-pck cost in fp64 read from global memory, as the reference's matrix is float64) and the PoseTrack CLEAR-MOT
+// accumulator (poseval.cu, fp64 costs as py-motmetrics hands scipy the fp64 distances).
 //
 // It restates the rectangular shortest augmenting path algorithm (Crouse 2016) in the exact order scipy >= 1.6 walks it
 // (see oracle/lsa.py, pinned live against the installed scipy):
@@ -58,10 +59,29 @@ __device__ __forceinline__ LsaSmemT<T> lsa_carve_t(unsigned char* base, int dvec
   return s;
 }
 
-// Solve on the internal (nr <= nc) matrix in s.C.  All 32 lanes participate.
-// On return col4row[i] (i < nr) holds the assignment.  Returns false if infeasible.
+// Internal (nr <= nc) matrix element (i, j) = C[i * rs + j * cs]: row-major in shared memory (rs = nc, cs = 1), or a
+// caller's [P, ldc] matrix in global memory read as it is (rs = ldc, cs = 1) or transposed (rs = 1, cs = ldc).
 template <typename T>
-__device__ bool lsa_solve_warp(const LsaSmemT<T>& s, int nr, int nc) {
+struct LsaRows {
+  const T* C;
+  size_t rs, cs;
+  __device__ __forceinline__ const T* row(int i) const { return C + (size_t)i * rs; }
+  __device__ __forceinline__ double at(const T* r, int j) const { return (double)r[(size_t)j * cs]; }
+};
+
+// The same with cs = 1 known at compile time (the shared-memory matrix).
+template <typename T>
+struct LsaDenseRows {
+  const T* C;
+  int nc;
+  __device__ __forceinline__ const T* row(int i) const { return C + (size_t)i * nc; }
+  __device__ __forceinline__ double at(const T* r, int j) const { return (double)r[j]; }
+};
+
+// Solve on the internal (nr <= nc) matrix `rows`.  All 32 lanes participate.
+// On return col4row[i] (i < nr) holds the assignment.  Returns false if infeasible.
+template <typename T, typename Rows>
+__device__ bool lsa_solve_warp_rows(const LsaSmemT<T>& s, const Rows& rows, int nr, int nc) {
   const int lane = threadIdx.x & 31;
   const unsigned FULL = 0xffffffffu;
   for (int x = lane; x < nr; x += 32) { s.u[x] = 0.0; s.col4row[x] = -1; }
@@ -76,12 +96,12 @@ __device__ bool lsa_solve_warp(const LsaSmemT<T>& s, int nr, int nc) {
     while (sink == -1) {
       if (lane == 0) s.SR[i] = 1;
       const double ui = s.u[i];
-      const T* ci = s.C + (size_t)i * nc;
+      const auto* ci = rows.row(i);
       double lmin = CUDART_INF;
       int lfirst = 0x7fffffff, lun = -1;
       for (int it = lane; it < num_remaining; it += 32) {
         const int j = s.remaining[it];
-        const double r = __dsub_rn(__dsub_rn(__dadd_rn(minVal, (double)ci[j]), ui), s.v[j]);
+        const double r = __dsub_rn(__dsub_rn(__dadd_rn(minVal, rows.at(ci, j)), ui), s.v[j]);
         double sp = s.spc[j];
         if (r < sp) { s.path[j] = i; s.spc[j] = r; sp = r; }
         const bool un = (s.row4col[j] == -1);
@@ -131,6 +151,12 @@ __device__ bool lsa_solve_warp(const LsaSmemT<T>& s, int nr, int nc) {
     __syncwarp();
   }
   return true;
+}
+
+// Solve on the internal (nr <= nc) row-major matrix in s.C.
+template <typename T>
+__device__ bool lsa_solve_warp(const LsaSmemT<T>& s, int nr, int nc) {
+  return lsa_solve_warp_rows(s, LsaDenseRows<T>{s.C, nc}, nr, nc);
 }
 
 }  // namespace dt

@@ -26,20 +26,19 @@ __device__ __forceinline__ double pck_cost_gt(const float* __restrict__ a, const
   return 1.0 - (double)cnt / (double)K;
 }
 
-// cost [F, dmax, dmax] (rows = GT, cols = detections) = fp32(fp32(w_iou * (1 - IoU)) + w_pck * pck) as
+// cost [F, dmax, dmax] fp64 (rows = GT, cols = detections) = fp32(w_iou * (1 - IoU)) + w_pck * pck as
 // _compute_distance_matrix sums its terms (tracking_engine.py:158-181); entries beyond the counts are 0.
 __global__ void gt_costs_kernel(const float* __restrict__ boxes, int ld, int T, const float* __restrict__ poses, int R, int K,
                                 int ht, int hb, double thr, const int* __restrict__ counts, int nframes, int dmax, float w_iou,
-                                double w_pck, float* __restrict__ cost) {
+                                double w_pck, double* __restrict__ cost) {
   const int f = blockIdx.x;
   const int P = min(counts[2 * f], dmax), Q = min(counts[2 * f + 1], dmax);
-  float* C = cost + (size_t)f * dmax * dmax;
+  double* C = cost + (size_t)f * dmax * dmax;
   const size_t ldp = (size_t)R * K;
   for (int e = threadIdx.x; e < dmax * dmax; e += blockDim.x) {
     const int p = e / dmax, q = e - p * dmax;
-    float c = 0.f;
+    double acc = 0.0;
     if (p < P && q < Q) {
-      double acc = 0.0;
       if (w_iou != 0.f) {
         const float* pb = boxes + ((size_t)(2 * f) * dmax + p) * ld;
         const float* qb = boxes + ((size_t)(2 * f + 1) * dmax + q) * ld;
@@ -50,9 +49,8 @@ __global__ void gt_costs_kernel(const float* __restrict__ boxes, int ld, int T, 
       if (w_pck != 0.0)
         acc = __dadd_rn(acc, __dmul_rn(pck_cost_gt(poses + ((size_t)(2 * f) * dmax + p) * ldp,
                                                    poses + ((size_t)(2 * f + 1) * dmax + q) * ldp, K, ht, hb, thr), w_pck));
-      c = __double2float_rn(acc);
     }
-    C[e] = c;
+    C[e] = acc;
   }
 }
 
@@ -129,7 +127,7 @@ using namespace dt;
 
 extern "C" int dt_gt_frame_costs(const float* boxes, int ld, int T, const float* poses, int R, int K, int head_top,
                                  int head_bottom, double dist_thresh, const int* counts, int nframes, int dmax, float w_iou,
-                                 double w_pck, float* cost, void* stream) {
+                                 double w_pck, double* cost, void* stream) {
   DT_CHECK_ARG(nframes >= 0 && dmax >= 1 && dmax <= DT_LSA_MAX_DIM && T >= 1 && T <= DT_MAX_T && ld >= 4 * T,
                "dt_gt_frame_costs: bad shape nframes=%d dmax=%d T=%d ld=%d (dmax <= %d)", nframes, dmax, T, ld, DT_LSA_MAX_DIM);
   DT_CHECK_ARG(w_pck == 0.0 || (poses && K >= 1 && R >= 2 && head_top >= 0 && head_top < K && head_bottom >= 0 &&

@@ -100,21 +100,23 @@ ALGOS ={'hungarian': 0, 'greedy': 1}
 
 
 def lsa_batched(cost, nrows, ncols, algo='hungarian'):
-    """cost [B, D, D'] cuda fp32 (rows prev, cols cur); returns matches [B, dmax] int32."""
+    """cost [B, D, D'] cuda (rows prev, cols cur): fp64 costs are solved in fp64 (dt_lsa_batched_f64), anything else as
+    fp32.  Returns (matches [B, dmax] int32, status [B] int32: 1 = infeasible or, for hungarian, a NaN / -inf entry)."""
     torch = L.require_cuda()
-    cost = _f32c(cost, torch)
+    f64 = cost.dtype == torch.float64
+    cost = cost.to(device='cuda').contiguous() if f64 else _f32c(cost, torch)
     B, P, Q = cost.shape
     dmax = max(P, Q)
     if P != dmax or Q != dmax:
-        pad = torch.zeros((B, dmax, dmax), dtype=torch.float32, device='cuda')
+        pad = torch.zeros((B, dmax, dmax), dtype=cost.dtype, device='cuda')
         pad[:, :P, :Q] = cost
         cost = pad
     nrows = nrows.to(device='cuda', dtype=torch.int32).contiguous()
     ncols = ncols.to(device='cuda', dtype=torch.int32).contiguous()
     matches = torch.empty((B, dmax), dtype=torch.int32, device='cuda')
     status = torch.empty((B,), dtype=torch.int32, device='cuda')
-    L.call('dt_lsa_batched', L.ptr(cost), B, dmax, dmax, L.ptr(nrows), L.ptr(ncols), ALGOS[algo], L.ptr(matches),
-           L.ptr(status), L.stream_ptr())
+    L.call('dt_lsa_batched_f64' if f64 else 'dt_lsa_batched', L.ptr(cost), B, dmax, dmax, L.ptr(nrows), L.ptr(ncols),
+           ALGOS[algo], L.ptr(matches), L.ptr(status), L.stream_ptr())
     return matches, status
 
 
@@ -146,7 +148,7 @@ def pose_pck_cost(a, b, head_top, head_bottom, dist_thresh=0.5):
 
 
 def frame_costs(boxes, counts, is_start, poses=None, T=1, w_iou=1.0, w_pck=0.0, head_top=2, head_bottom=1, dist_thresh=0.5):
-    """boxes [F, Dmax, ld], poses [F, Dmax, 4|3, K] (or None) -> cost [F, Dmax, Dmax] fp32 (rows = previous frame)."""
+    """boxes [F, Dmax, ld], poses [F, Dmax, 4|3, K] (or None) -> cost [F, Dmax, Dmax] fp64 (rows = previous frame)."""
     torch = L.require_cuda()
     boxes = _f32c(boxes, torch)
     F, dmax, ld = boxes.shape
@@ -157,7 +159,7 @@ def frame_costs(boxes, counts, is_start, poses=None, T=1, w_iou=1.0, w_pck=0.0, 
     if poses is not None:
         poses = _f32c(poses, torch)
         K, ldp = poses.shape[3], poses.shape[2] * poses.shape[3]
-    cost = torch.empty((F, dmax, dmax), dtype=torch.float32, device='cuda')
+    cost = torch.empty((F, dmax, dmax), dtype=torch.float64, device='cuda')
     L.call('dt_frame_costs', L.ptr(boxes), ld, T, L.ptr(poses), ldp, K, int(head_top), int(head_bottom), float(dist_thresh),
            L.ptr(counts), L.ptr(is_start), F, dmax, float(w_iou), float(w_pck), L.ptr(cost), L.stream_ptr())
     return cost
@@ -193,7 +195,7 @@ def prune_detections(boxes, counts, hw, conf, T=1, center_only=True, min_area=50
 
 def gt_frame_costs(boxes, counts, poses=None, T=1, w_iou=1.0, w_pck=0.0, head_top=2, head_bottom=1, dist_thresh=0.5):
     """boxes [2F, Dmax, ld], poses [2F, Dmax, R, K] (or None): the GT of frame f at entry 2f, its detections at 2f + 1 ->
-    cost [F, Dmax, Dmax] fp32, rows = GT (tracking_engine.py:287-296 with the frame's GT as the previous frame)."""
+    cost [F, Dmax, Dmax] fp64, rows = GT (tracking_engine.py:287-296 with the frame's GT as the previous frame)."""
     torch = L.require_cuda()
     boxes = _f32c(boxes, torch)
     F2, dmax, ld = boxes.shape
@@ -202,7 +204,7 @@ def gt_frame_costs(boxes, counts, poses=None, T=1, w_iou=1.0, w_pck=0.0, head_to
     if poses is not None:
         poses = _f32c(poses, torch)
         R, K = poses.shape[2], poses.shape[3]
-    cost = torch.empty((F2 // 2, dmax, dmax), dtype=torch.float32, device='cuda')
+    cost = torch.empty((F2 // 2, dmax, dmax), dtype=torch.float64, device='cuda')
     L.call('dt_gt_frame_costs', L.ptr(boxes), ld, T, L.ptr(poses), R, K, int(head_top), int(head_bottom), float(dist_thresh),
            L.ptr(counts), F2 // 2, dmax, float(w_iou), float(w_pck), L.ptr(cost), L.stream_ptr())
     return cost

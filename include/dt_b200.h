@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define DT_B200_ABI_VERSION 3
+#define DT_B200_ABI_VERSION 4
 #define DT_MAX_T 8              /* frames per tube supported by the box kernels */
 #define DT_NMS_MAX_BOXES 8192   /* per problem */
 #define DT_LSA_MAX_DIM 224      /* max(prev, cur) detections per frame pair */
@@ -103,10 +103,14 @@ int dt_box_vote(const float* top, const int* top_keep, const int* top_counts, in
  * lib/core/tracking_engine.py:237, batched: cost [batch, dmax, ldc] fp32
  * (rows = previous frame, cols = current frame), nrows/ncols [batch] device.
  * matches [batch, dmax]: matches[q] = assigned row p, or -1
- * (tracking_engine.py:229-246).  status [batch] (may be NULL): 1 = infeasible.
- * Indices equal scipy >= 1.6 bit-for-bit (see oracle/lsa.py). */
+ * (tracking_engine.py:229-246).  status [batch] (may be NULL): 1 = infeasible, or (hungarian) a NaN or -inf entry,
+ * where scipy raises ValueError.  Indices equal scipy >= 1.6 bit-for-bit (see oracle/lsa.py). */
 int dt_lsa_batched(const float* cost, int batch, int dmax, int ldc, const int* nrows,
                    const int* ncols, int algo, int* matches, int* status, void* stream);
+/* The same on fp64 costs [batch, dmax, ldc >= dmax] (dt_frame_costs / dt_gt_frame_costs), solved in fp64 as scipy
+ * solves the reference's float64 matrix.  The costs are read from global memory, not staged in shared memory. */
+int dt_lsa_batched_f64(const double* cost, int batch, int dmax, int ldc, const int* nrows,
+                       const int* ncols, int algo, int* matches, int* status, void* stream);
 
 /* lib/core/tracking_engine.py:158-246 fused: cost = weight * (1 - IoU) between
  * frame f-1 and frame f, then the assignment.  frames [nframes, dmax, ld]
@@ -122,15 +126,14 @@ int dt_match_frames(const float* frames, int nframes, int dmax, int ld, int T, c
 int dt_pose_pck_cost(const float* a, int P, const float* b, int Q, int ld, int K, int head_top, int head_bottom,
                      float dist_thresh, double* out, void* stream);
 
-/* lib/core/tracking_engine.py:158-181 for all frame pairs at once: cost [nframes, dmax, dmax] fp32 with
- * cost[f][p][q] = fp32(w_iou * (1 - IoU(boxes[f-1][p], boxes[f][q])) + w_pck * pck(poses[f-1][p], poses[f][q])) (fp64 sum, like
- * np.sum(np.stack(all_Cs))); frames with is_start != 0 (and frame 0) and entries beyond counts are 0.  boxes [nframes, dmax,
- * ldb], poses [nframes, dmax, ldp] (may be NULL when w_pck == 0).  Feed to dt_lsa_batched (nrows = counts[f-1] or 0, ncols =
- * counts[f]).  The reference solves the fp64 sum; here it is rounded to fp32 first (identical indices unless two
- * assignments' total costs differ by less than 1e-7). */
+/* lib/core/tracking_engine.py:158-181 for all frame pairs at once: cost [nframes, dmax, dmax] fp64 with
+ * cost[f][p][q] = fp32(w_iou * (1 - IoU(boxes[f-1][p], boxes[f][q]))) + w_pck * pck(poses[f-1][p], poses[f][q]) (fp64 sum,
+ * like np.sum(np.stack(all_Cs))); frames with is_start != 0 (and frame 0) and entries beyond counts are 0.  boxes [nframes,
+ * dmax, ldb], poses [nframes, dmax, ldp] (may be NULL when w_pck == 0).  Feed to dt_lsa_batched_f64 (nrows = counts[f-1] or
+ * 0, ncols = counts[f]): the reference solves this fp64 sum, and rounding it to fp32 would break its exact ties differently. */
 int dt_frame_costs(const float* boxes, int ldb, int T, const float* poses, int ldp, int K, int head_top, int head_bottom,
                    float dist_thresh, const int* counts, const unsigned char* is_start, int nframes, int dmax, float w_iou,
-                   double w_pck, float* cost, void* stream);
+                   double w_pck, double* cost, void* stream);
 
 /* ---- upper_bound.cu: TRACKING.DEBUG.UPPER_BOUND* (lib/core/tracking_engine.py:272-350) ---- */
 #define DT_UB_COMPACT 1     /* UPPER_BOUND: keep the detections a GT took, with the GT's track id */
@@ -139,11 +142,11 @@ int dt_frame_costs(const float* boxes, int ldb, int T, const float* poses, int l
 
 /* GT-vs-detection cost matrices of every frame: boxes [2 * nframes, dmax, ld] and poses [2 * nframes, dmax, R, K] hold the
  * GT of frame f at entry 2f (boxes padded with a score column, integer-valued keypoints in rows 0..2) and its detections at
- * entry 2f + 1; counts [2 * nframes].  cost [nframes, dmax, dmax] fp32, rows = GT, = fp32(fp32(w_iou * (1 - IoU)) + w_pck *
- * pck) with the pck term in fp64 (numpy promotes the reference's int32 GT keypoints so); 0 beyond the counts.  Feed to
- * dt_lsa_batched with nrows = counts[2f], ncols = counts[2f + 1]. */
+ * entry 2f + 1; counts [2 * nframes].  cost [nframes, dmax, dmax] fp64, rows = GT, = fp32(w_iou * (1 - IoU)) + w_pck * pck
+ * with the pck term in fp64 (numpy promotes the reference's int32 GT keypoints so); 0 beyond the counts.  Feed to
+ * dt_lsa_batched_f64 with nrows = counts[2f], ncols = counts[2f + 1]. */
 int dt_gt_frame_costs(const float* boxes, int ld, int T, const float* poses, int R, int K, int head_top, int head_bottom,
-                      double dist_thresh, const int* counts, int nframes, int dmax, float w_iou, double w_pck, float* cost,
+                      double dist_thresh, const int* counts, int nframes, int dmax, float w_iou, double w_pck, double* cost,
                       void* stream);
 /* One CTA per frame of the same packing: matches [nframes, ldm] (detection -> GT row or -1, the configured cost; needed
  * with DT_UB_COMPACT) and matches_gt [nframes, ldmg] (the bbox Hungarian match of UPPER_BOUND_5_GT_KPS_ONLY, may be NULL).

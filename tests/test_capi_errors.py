@@ -88,3 +88,22 @@ def test_every_compute_entry_point_has_an_error_case():
     covered = {c[0] for c in _cases()}
     host_only = {'dt_abi_version', 'dt_nms_workspace_bytes', 'dt_rpn_workspace_bytes', 'dt_rpn_targets_workspace_bytes'}
     assert set(L.SIGNATURES) - host_only <= covered, set(L.SIGNATURES) - host_only - covered
+
+
+def test_lsa_batched_f64_argument_checks():
+    """dt_lsa_batched_f64 (the fp64 solver of the pose-pck tracking cost) rejects bad shapes, algos and null pointers on
+    the host; an empty batch is a no-op."""
+    lib = L.lib()
+    cases = [
+        ((None, 1, 225, 225, None, None, 0, None, None, None), b'dmax=225'),
+        ((None, 1, 0, 1, None, None, 0, None, None, None), b'dmax=0'),
+        ((None, 1, 100, 99, None, None, 0, None, None, None), b'ldc=99'),
+        ((None, -1, 8, 8, None, None, 0, None, None, None), b'batch=-1'),
+        ((None, 1, 8, 8, None, None, 2, None, None, None), b'unknown algo 2'),
+        ((None, 1, 8, 8, None, None, 0, None, None, None), b'null pointer'),
+    ]
+    for args, msg in cases:
+        rc = lib.dt_lsa_batched_f64(*args)
+        assert rc != 0, args
+        assert msg in lib.dt_last_error(), (args, lib.dt_last_error())
+    assert lib.dt_lsa_batched_f64(None, 0, 8, 8, None, None, 0, None, None, None) == 0

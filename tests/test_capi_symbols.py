@@ -33,7 +33,7 @@ def test_ctypes_table_matches_header():
 
 def test_abi_version_and_error_channel():
     lib = _lib.lib()
-    assert lib.dt_abi_version() == 3
+    assert lib.dt_abi_version() == 4
     # argument validation happens on the host before any CUDA call: usable without a GPU
     rc = lib.dt_bbox_overlaps(None, 4, 4, None, 4, 4, 99, None, 4, None)
     assert rc != 0
