@@ -11,10 +11,21 @@ Tolerances (north star: 1e-3 relative fp32):
   bf16x3   : [hi | lo] bf16 pairs, 3 bf16 MMAs per k-block (the headline parity mode; operands carry 16 mantissa
              bits, 2^-17 relative): |err| <= 1e-4 * max|y| for both the bf16-pair output and the plain fp32 output.
 """
+import zlib
+
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
+
+
+def with_operands(argnames, cases, ids):
+    """parametrize a value test over `cases` (tuples of `argnames`) with random operands under their own ids, then over
+    each case again with operands='integer' (id + '-integer'): the exact forward check as one more input of the test."""
+    cases = [c if isinstance(c, tuple) else (c,) for c in cases]
+    return pytest.mark.parametrize(argnames + ',operands',
+                                   [c + ('random',) for c in cases] + [c + ('integer',) for c in cases],
+                                   ids=list(ids) + ['%s-integer' % i for i in ids])
 
 
 def _ref_conv(x, w, stride, pad, scale, bias, residual, res_mode, relu):
@@ -223,22 +234,69 @@ def test_conv_rejects_bad_arguments():
         cv.conv3d(x, wp, (1, 1, 1), cin=12)
 
 
-@pytest.mark.parametrize('mode', ['bf16', 'tf32', 'bf16x3'])
-def test_conv1_packed_rows_vs_torch(mode):
+@with_operands('mode', ['bf16', 'tf32', 'bf16x3'], ['bf16', 'tf32', 'bf16x3'])
+def test_conv1_packed_rows_vs_torch(mode, operands):
     """dt_conv1_7x7s2 (filter row packed into K over a zero-bordered blob) == conv 7x7 s2 p3 + affine + relu."""
-    _check_conv1_packed_rows(mode, 3, 64, 96)
+    _check_conv1_packed_rows(mode, 3, 64, 96, operands)
 
 
-@pytest.mark.parametrize('mode', ['bf16', 'tf32', 'bf16x3'])
-def test_conv1_packed_rows_three_tiles_per_cta(mode):
+@with_operands('mode', ['bf16', 'tf32', 'bf16x3'], ['bf16', 'tf32', 'bf16x3'])
+def test_conv1_packed_rows_three_tiles_per_cta(mode, operands):
     """The same at three 256 x 336 frames: every CTA walks at least three 128-row tiles."""
     import torch
     Fr, H, W = 3, 256, 336
     assert Fr * (H // 2) * (W // 2) / 128 >= 3 * torch.cuda.get_device_properties(0).multi_processor_count
-    _check_conv1_packed_rows(mode, Fr, H, W)
+    _check_conv1_packed_rows(mode, Fr, H, W, operands)
 
 
-def _check_conv1_packed_rows(mode, Fr, H, W):
+def _check_conv1_exact(mode, Fr, H, W):
+    """The tensor-core conv1 variants on integer blobs and filters, bit for bit: bf16 with fp32 and with bf16 outputs, tf32
+    with tf32-rounded fp32 outputs, and bf16x3 on independent integer [hi3 | lo3 | 0 0] pixels with W_hi / W_lo blocks laid
+    out as dt_conv1_7x7s2 reads them, whose bf16-pair output must be (x_hi + x_lo) W_hi + x_hi W_lo rounded as the
+    epilogue does."""
+    import torch
+    from detectandtrack_b200.ops import conv as cv
+    g = torch.Generator(device='cuda').manual_seed(zlib.crc32(('conv1/%s/%d' % (mode, H)).encode()))
+    split = mode == 'bf16x3'
+    a = int_amplitude(147, 'tf32' if mode == 'tf32' else 'bf16')
+    cp = 4 if mode == 'tf32' else 8
+    store = torch.float32 if mode == 'tf32' else torch.bfloat16
+
+    def ints(shape):
+        return torch.randint(-a, a + 1, shape, generator=g, device='cuda').float()
+    xs = [ints((Fr, 1, H, W, 3)) for _ in range(1 + split)]
+    ws = [ints((64, 3, 1, 7, 7)) for _ in range(1 + split)]
+    blob = torch.zeros((Fr, H + 6, W + 8, cp), device='cuda')              # the zero border of dt_prep_clip(border=(3, 4))
+    for i, xi in enumerate(xs):
+        blob[:, 3:3 + H, 4:4 + W, 3 * i:3 * i + 3] = xi[:, 0]
+    x = blob.view(Fr, (H + 6) // 2, 2, W + 8, cp).permute(0, 2, 1, 3, 4).to(store).contiguous()  # row r at [r & 1][r >> 1]
+    wk = [w[:, :, 0].permute(2, 0, 3, 1) for w in ws]                        # (kh, Cout, kw, c)
+    if split:                                      # block 2 kh = [W_hi | W_hi] per pixel, block 2 kh + 1 = [W_lo | 0]
+        wp = torch.zeros((7, 2, 64, 8, 8), device='cuda')
+        wp[:, 0, :, :7, 0:3] = wk[0]
+        wp[:, 0, :, :7, 3:6] = wk[0]
+        wp[:, 1, :, :7, 0:3] = wk[1]
+        wp = wp.reshape(14, 64, 64)
+    else:
+        wp = torch.zeros((7, 64, 8, cp), device='cuda')
+        wp[:, :, :7, :3] = wk[0]
+        wp = wp.reshape(7, 64, 8 * cp)
+    wp = wp.to(store).contiguous()
+    sc = torch.tensor(SCALES, device='cuda')[torch.randint(0, len(SCALES), (64,), generator=g, device='cuda')]
+    bi = torch.randint(-256, 257, (64,), generator=g, device='cuda').float() / 4
+    ref = dict(xs=xs, ws=ws, scale=sc, bias=bi, res=[], res_mode=0, relu=True, a=a, K=147, split=split, bk=3)
+    dtype = cv.MODE_NAMES[mode]
+    runs = {'bf16': [('f32', True), ('bf16', None)], 'tf32': [('f32 tf32', None)], 'bf16x3': [('bf16 pair', None)]}[mode]
+    for kind, out_f32 in runs:
+        y = cv.conv1_7x7s2(x, wp, (H, W), sc, bi, relu=True, dtype=dtype, out_f32=out_f32)
+        ref['kind'] = kind
+        msg = _exact_mismatch(y[:, None], ref, (1, 2, 2), (0, 3, 3), 'conv1 %s %s' % (mode, kind))
+        assert msg is None, msg
+
+
+def _check_conv1_packed_rows(mode, Fr, H, W, operands='random'):
+    if operands == 'integer':
+        return _check_conv1_exact(mode, Fr, H, W)
     import torch
     import torch.nn.functional as F
     from detectandtrack_b200.ops import conv as cv, dense_ops
@@ -319,7 +377,8 @@ def test_pairs_to_f16_rounds_and_saturates_like_torch():
 
 # ------------------------------------------------------------------ every conv plan of the benchmarked step, multi-tile
 from test_conv_plan import R50_FPN_3D, REDUCED, conv_args, layer_modes, step_plan  # noqa: E402
-from test_conv_reference import conv_ref  # noqa: E402
+from test_conv_reference import (EXACT_LIMIT, SCALES, conv_ref, exact_bound, exact_epilogue, exact_store,  # noqa: E402
+                                 exact_terms, int_amplitude, operand_format, same_bits, term_contributions, upsample_res)
 
 STEP_CASES = [(l, m) for l in R50_FPN_3D for m in layer_modes(l)]
 # DESIGN.md §4, max-norm.  bf16 / f16: the reference gets the same rounded operands, so only the fp32 accumulation order
@@ -345,10 +404,11 @@ def _epilogue(name):
     return False, name.startswith(('rpn conv', 'fc6', 'fc7', 'keypoint head'))
 
 
-def _step_inputs(layer, mode, g, shapes=None):
+def _step_inputs(layer, mode, g, shapes=None, operands='random'):
     """Device tensors of one layer at its reduced shape (in `shapes`, default REDUCED), stored the way the engine stores
     them in `mode`, and the values the kernel reads from them (rounded operands, hi + lo pairs, the stored residual) for
-    the reference."""
+    the reference.  operands='integer': independent integer hi / lo halves written straight into the stored rows
+    (_integer_operands), and for the reference the halves themselves and the output storage kind."""
     import torch
     from detectandtrack_b200.ops import conv as cv, dense_ops
     name, _, _, _, _, Cin, Cout, k, s, p, rm = layer
@@ -357,6 +417,20 @@ def _step_inputs(layer, mode, g, shapes=None):
     dt = cv.F16 if mode == 'f16' else cv.MODE_NAMES[mode]
     split = dt in cv.SPLIT_MODES
     affine, relu = _epilogue(name)
+    head = Cout % 64 != 0
+    if operands == 'integer':
+        res_dtype = torch.bfloat16 if mode in ('bf16', 'bf16x3') else torch.float32
+        xd, wp, scale, bias, res, ref = _integer_operands(g, (N, T, H, W), Cin, Cout, k, mode, affine,
+                                                          (N, To, Ho // rm, Wo // rm, Cout) if rm else None, res_dtype, split)
+        out = None
+        if head:                                   # fp32 head outputs in a padded row whose padding keeps a sentinel
+            out = torch.full((N, To, Ho, Wo, (Cout + 3) // 4 * 4), float('nan'), dtype=torch.float32, device='cuda')
+        kind = 'f32' if head else {'bf16': 'bf16', 'tf32': 'f32 tf32', 'tf32x3': 'tf32 pair', 'bf16x3': 'bf16 pair',
+                                   'f16': 'bf16 pair'}[mode]
+        run = dict(x=xd, w=wp, k=k, s=s, p=p, scale=scale, bias=bias, res=res, rm=rm, relu=relu, dtype=dt, out=out,
+                   out_f32=True if head else None, split_out=True if mode == 'f16' else None)
+        ref.update(res_mode=rm, relu=relu, kind=kind)
+        return run, ref
     x = torch.randn((N, T, H, W, Cin), generator=g, device='cuda')
     w = torch.randn((Cout, Cin) + k, generator=g, device='cuda') * (2.0 / (Cin * k[0] * k[1] * k[2])) ** 0.5
     scale = torch.rand(Cout, generator=g, device='cuda') + 0.5 if affine else None
@@ -377,7 +451,6 @@ def _step_inputs(layer, mode, g, shapes=None):
     if res is not None:
         res = cv.split_for(dt, res) if split else (res.bfloat16() if mode == 'bf16' else res)
     resr = None if res is None else (cv.join_split(res) if split else res.float())
-    head = Cout % 64 != 0
     out = None
     if head:                                       # final fp32 head outputs, in a row padded to 16 bytes as the engine does
         out = torch.empty((N, To, Ho, Wo, (Cout + 3) // 4 * 4), dtype=torch.float32, device='cuda')
@@ -385,6 +458,121 @@ def _step_inputs(layer, mode, g, shapes=None):
                out_f32=True if head else None, split_out=True if mode == 'f16' else None)
     ref = dict(x=xr, w=wr, scale=scale, bias=bias, residual=resr, res_mode=rm, relu=relu)
     return run, ref
+
+
+def _integer_operands(g, nthw, Cin, Cout, k, mode, affine, res_shape=None, res_dtype=None, res_split=False):
+    """Integer operands of one conv (test_conv_reference: the exact forward check): x, w and the residual in [-a, a]
+    (int_amplitude of the K = taps * Cin term sum), in the split modes independent hi and lo halves written straight
+    into the stored rows ([hi | lo] activations, packed filters [taps, Cout, 2 Cp] = cat([hi, lo], -1), not through
+    pack_weight); the AffineChannel scale a power of two, the bias a multiple of 1/4.  Returns the device tensors
+    (x, packed w, scale, bias, residual) and the reference inputs: the halves xs, ws ([Cout, Cin, kT, kH, kW]), res."""
+    import torch
+    import torch.nn.functional as F
+    from detectandtrack_b200.ops import conv as cv
+    split = mode in ('tf32x3', 'bf16x3')
+    fmt = operand_format(mode)
+    taps = k[0] * k[1] * k[2]
+    a = int_amplitude(taps * Cin, fmt)
+    store = {'bf16': torch.bfloat16, 'f16': torch.float16, 'tf32': torch.float32}[fmt]
+
+    def ints(shape):
+        return torch.randint(-a, a + 1, shape, generator=g, device='cuda').float()
+    xs = [ints(tuple(nthw) + (Cin,)) for _ in range(1 + split)]
+    wt = [ints((taps, Cout, Cin)) for _ in range(1 + split)]
+    Cp = -(-Cin // (4 if fmt == 'tf32' else 8)) * (4 if fmt == 'tf32' else 8)
+    xd = torch.cat(xs, -1).to(store).contiguous()
+    wp = torch.cat([F.pad(w, (0, Cp - Cin)) for w in wt], -1).to(store).contiguous()
+    ws = [w.reshape(k + (Cout, Cin)).permute(3, 4, 0, 1, 2) for w in wt]
+    scale = None
+    if affine:
+        scale = torch.tensor(SCALES, device='cuda')[torch.randint(0, len(SCALES), (Cout,), generator=g, device='cuda')]
+    bias = torch.randint(-256, 257, (Cout,), generator=g, device='cuda').float() / 4
+    res, rs = None, []
+    if res_shape is not None:
+        rs = [ints(res_shape) for _ in range(1 + res_split)]
+        res = torch.cat(rs, -1).to(res_dtype).contiguous()
+    assert torch.equal(xd.float(), torch.cat(xs, -1)) and (res is None or torch.equal(res.float(), torch.cat(rs, -1)))
+    return xd, wp, scale, bias, res, dict(xs=xs, ws=ws, scale=scale, bias=bias, res=rs, a=a, K=taps * Cin, split=split,
+                                          bk=64 if store != torch.float32 else 32)
+
+
+def _stored_cout(y, kind):
+    return y.shape[-1] // 2 if kind.endswith('pair') else y.shape[-1]
+
+
+def _exact_mismatch(y, ref, stride, pad, what, o=None, frames=None, hard=True):
+    """The exact forward check of one launch: y (as stored: bf16 rows, [hi | lo] pairs, fp32) against the emulation of
+    test_conv_reference on the integer operands `ref` (_integer_operands), bit for bit with +0 == -0.  frames = (first,
+    count) for an out_frames launch.  With `hard`, first asserts the fixture can see what it is for.  Returns None, or a
+    report: the first wrong element with its tile / CTA (o the plan), the difference, and each single (tap, k-block,
+    product) whose contribution, dropped or added once more, gives exactly the device value."""
+    import torch
+    xs, ws, kind, rm = ref['xs'], ref['ws'], ref['kind'], ref['res_mode']
+    scale, bias = ref['scale'], ref['bias']
+    smax = 1.0 if scale is None else float(scale.max())
+    bound = exact_bound(ref['a'], ref['K'], ref['split'], smax, float(bias.abs().max()) if bias is not None else 0.0,
+                        ref['a'] if ref['res'] else 0)
+    assert bound < EXACT_LIMIT, (what, bound)
+    terms = exact_terms(xs, ws, stride, pad)
+    t0 = 0
+    if frames:
+        t0 = frames[0]
+        terms = {n: v[:, t0:t0 + frames[1]] for n, v in terms.items()}
+    acc = sum(terms.values())
+    res = [upsample_res(r, rm) for r in ref['res']]
+    v = exact_epilogue(acc, scale, bias, res, ref['relu'])
+    want = exact_store(v, kind)
+    Cout = acc.shape[-1]
+    pair = kind.endswith('pair')
+
+    def differs(a, b):                             # per output element (either half of a pair)
+        d = ~same_bits(a, b)
+        return d[..., :Cout] | d[..., Cout:] if pair else d
+    if hard:
+        if kind == 'bf16':
+            bits = v.float().view(torch.int32) & 0xFFFF
+            assert bool((v.abs() > 256).any()) and int((bits == 0x8000).sum()) >= 1, (what, 'no bf16 rounding at ties')
+        if pair:
+            assert bool((want[..., Cout:] != 0).any()), (what, 'lo halves all zero')
+        if ref['split']:                           # the neighbouring arithmetics differ in most outputs ReLU leaves
+            live = v != 0
+            lolo = conv_ref(xs[1], ws[1], stride, pad)
+            if frames:
+                lolo = lolo[:, t0:t0 + frames[1]]
+            for n, wrong in (('lo*lo added', acc + lolo), ('x_lo*w_hi dropped', acc - terms['x_lo*w_hi']),
+                             ('x_hi*w_lo dropped', acc - terms['x_hi*w_lo'])):
+                d = differs(exact_store(exact_epilogue(wrong, scale, bias, res, ref['relu']), kind), want)
+                assert float(d[live].double().mean()) > 0.5, (what, n)
+    assert y.shape == want.shape and y.dtype == want.dtype, (what, y.shape, want.shape, y.dtype, want.dtype)
+    bad = differs(y, want)
+    if not bool(bad.any()):
+        return None
+    nbad = int(bad.sum())
+    idx = [int(i) for i in torch.unravel_index(bad.view(-1).nonzero()[0, 0], bad.shape)]
+    n, t, h, w, c = idx
+    cols = [c, c + Cout] if pair else [c]
+
+    def value(s):                                  # a stored element as a number (hi + lo for pairs)
+        return float(s.double().sum())
+    got = y[n, t, h, w, cols]
+    msg = '%s: %d wrong outputs; first at %s' % (what, nbad, idx)
+    if o is not None:
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+        msg += ' (%s)' % _locate(idx, tuple(acc.shape), o, sms)
+    msg += ': got %r, want %r (difference %r)' % (value(got), value(want[n, t, h, w, cols]),
+                                                  value(got) - value(want[n, t, h, w, cols]))
+    contrib = term_contributions(xs, ws, stride, pad, (n, t + t0, h, w, c), ref['bk'])
+    e_res = [r[n, t, h, w, c:c + 1] for r in res]
+    sc = None if scale is None else scale[c:c + 1]
+    bi = None if bias is None else bias[c:c + 1]
+    hits = []
+    for key, val in contrib.items():
+        for sign, verb in ((-1, 'dropped'), (1, 'added twice')):
+            cand = exact_store(exact_epilogue(acc[n, t, h, w, c:c + 1] + sign * val, sc, bi, e_res, ref['relu']), kind)
+            if val != 0 and bool(same_bits(cand, got).all()):
+                hits.append('%s of tap %s, k-block %d %s' % (key[2], key[0], key[1], verb))
+    msg += '; equals a single term: %s' % ('; '.join(hits) if hits else 'none of the %d' % len(contrib))
+    return msg
 
 
 def _locate(idx, shape, o, sms):
@@ -399,28 +587,44 @@ def _locate(idx, shape, o, sms):
             % (m, n // o.TB, t // o.TT, h // o.TH, w // o.TW, c // o.BN, tile, tile // sms, tile % sms))
 
 
-@pytest.mark.parametrize('layer,mode', STEP_CASES, ids=['%s-%s' % (l[0], m) for l, m in STEP_CASES])
-def test_step_layer_over_three_waves_vs_fp64(layer, mode, record_property):
+@with_operands('layer,mode', STEP_CASES, ['%s-%s' % (l[0], m) for l, m in STEP_CASES])
+def test_step_layer_over_three_waves_vs_fp64(layer, mode, operands, record_property):
     """Every (layer, mode) of the benchmarked step at its reduced shape (test_conv_plan.REDUCED: the step's plan, three
     or more tiles per CTA, a ragged last wave) with the engine's storage and epilogue, against the fp64 tap-sum
-    reference on the values the kernel reads.  bf16 outputs: |y - ref| <= 2^-8 |ref| + 2e-4 max|ref| elementwise (half a
-    bf16 ulp of output rounding plus the accumulation-order error); the others _step_tol * max|ref|."""
-    _check_step_case(layer, mode, step_plan(layer, mode, reduced=True), None, '%s/%s' % (layer[0], mode), record_property)
+    reference on the values the kernel reads.  Random operands: bf16 outputs |y - ref| <= 2^-8 |ref| + 2e-4 max|ref|
+    elementwise (half a bf16 ulp of output rounding plus the accumulation-order error); the others _step_tol * max|ref|.
+    Integer operands: bit for bit (_exact_mismatch)."""
+    _check_step_case(layer, mode, step_plan(layer, mode, reduced=True), None, '%s/%s' % (layer[0], mode), record_property,
+                     operands)
 
 
-def _check_step_case(layer, mode, o, shapes, seed_tag, record_property):
-    """One table row at its reduced shape (`shapes`, default REDUCED; `o` its plan) through cv.conv3d, against conv_ref:
-    the body of test_step_layer_over_three_waves_vs_fp64, shared with tests/test_gpu_conv_workloads.py."""
-    import zlib
+def _check_step_case(layer, mode, o, shapes, seed_tag, record_property, operands='random'):
+    """One table row at its reduced shape (`shapes`, default REDUCED; `o` its plan) through cv.conv3d, against conv_ref
+    (random operands) or the exact emulation (integer operands): the body of test_step_layer_over_three_waves_vs_fp64,
+    shared with tests/test_gpu_conv_workloads.py."""
     import torch
     from detectandtrack_b200.ops import conv as cv
     name, Cout = layer[0], layer[6]
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     assert o.tiles / sms >= 3, (name, mode, o.tiles, sms)
     g = torch.Generator(device='cuda').manual_seed(zlib.crc32(seed_tag.encode()))
-    run, ref_in = _step_inputs(layer, mode, g, shapes)
+    run, ref_in = _step_inputs(layer, mode, g, shapes, operands)
     y = cv.conv3d(run['x'], run['w'], run['k'], run['s'], run['p'], run['scale'], run['bias'], run['res'], run['rm'],
                   run['relu'], out_f32=run['out_f32'], dtype=run['dtype'], out=run['out'], split_out=run['split_out'])
+    record_property('tiles', o.tiles)
+    record_property('tiles_per_cta', round(o.tiles / sms, 2))
+    if operands == 'integer':
+        if run['out'] is not None:
+            # the row padding past Cout (to the end of the 16-byte unit holding channel Cout - 1) is stored with the
+            # whole unit, from accumulators of zero weight rows with scale 1 and bias 0: zeros, never the sentinel or
+            # a stray value
+            pad = run['out'][..., Cout:]
+            assert bool((pad == 0).all()), (name, mode, 'padding channels', pad.unique()[:8].tolist())
+            y = y[..., :Cout]
+        msg = _exact_mismatch(y, ref_in, layer[8], layer[9], '%s %s' % (name, mode), o)
+        if msg:
+            pytest.fail(msg)
+        return
     if run['out'] is not None:
         y = y[..., :Cout]
     elif run['split_out'] or run['dtype'] in cv.SPLIT_MODES:
@@ -434,31 +638,66 @@ def _check_step_case(layer, mode, o, shapes, seed_tag, record_property):
     bound = 2 ** -8 * ref.abs() + 2e-4 * den if bf16_out else _step_tol(layer, mode) * den
     ratio = err / bound
     worst = ratio.max().item()
-    record_property('tiles', o.tiles)
-    record_property('tiles_per_cta', round(o.tiles / sms, 2))
     record_property('worst_err_over_tol', worst)
     if not worst <= 1.0:                           # NaN too: a wrong shared-memory read can produce it
         idx = [int(i) for i in torch.unravel_index(ratio.argmax(), ratio.shape)]
         pytest.fail('%s %s: error %.3g x the bound at %s, %s' % (name, mode, worst, idx, _locate(idx, y.shape, o, sms)))
 
 
-@pytest.mark.parametrize('mode', ['bf16x3', 'f16'])
-def test_posthoc_fpn_time_major_and_center_frame_vs_fp64(mode):
+@with_operands('mode', ['bf16x3', 'f16'], ['bf16x3', 'f16'])
+def test_posthoc_fpn_time_major_and_center_frame_vs_fp64(mode, operands):
     """The post-hoc FPN conv as the slice-center link runs it: frames-outermost output (time_major) and the centre
-    output frame alone (out_frames=(1, 1)), in bf16x3 and with fp16 operands writing bf16 pairs (bf16x3h)."""
+    output frame alone (out_frames=(1, 1)), in bf16x3 and with fp16 operands writing bf16 pairs (bf16x3h); on integer
+    operands bit for bit."""
     import torch
     from detectandtrack_b200.ops import conv as cv
     layer = next(l for l in R50_FPN_3D if l[0] == 'fpn post-hoc P4')
     g = torch.Generator(device='cuda').manual_seed(14)
-    run, ref_in = _step_inputs(layer, mode, g)
-    ref = conv_ref(ref_in['x'], ref_in['w'], layer[8], layer[9], None, ref_in['bias'])
+    run, ref_in = _step_inputs(layer, mode, g, operands=operands)
     kw = dict(dtype=run['dtype'], split_out=run['split_out'])
     tm = cv.conv3d(run['x'], run['w'], run['k'], run['s'], run['p'], None, run['bias'], time_major=True, **kw)
     mid = cv.conv3d(run['x'], run['w'], run['k'], run['s'], run['p'], None, run['bias'], out_frames=(1, 1), **kw)
     assert not tm.is_contiguous() and tm[:, 1:2].is_contiguous() and mid.shape[1] == 1
+    if operands == 'integer':
+        for y, frames, what in ((tm, None, 'time_major'), (mid, (1, 1), 'out_frames=(1, 1)')):
+            msg = _exact_mismatch(y, ref_in, layer[8], layer[9], '%s %s %s' % (layer[0], mode, what), frames=frames)
+            assert msg is None, msg
+        return
+    ref = conv_ref(ref_in['x'], ref_in['w'], layer[8], layer[9], None, ref_in['bias'])
     tol = STEP_TOL[mode] * ref.abs().max().item()
     assert (cv.join_split(tm).double() - ref).abs().max().item() <= tol
     assert (cv.join_split(mid).double() - ref[:, 1:2]).abs().max().item() <= tol
+
+
+@pytest.mark.parametrize('mode', ['bf16x3', 'tf32x3'])
+def test_exact_check_names_a_wrong_lo_box(mode, monkeypatch):
+    """Negative control of the exact check: activation rows [hi | lo | lo'] with the descriptor's in_lo_off at lo', lo'
+    being lo with k-block 1 zeroed, against the reference built from lo.  The launch is legal and reads a wrong lo box;
+    the check must report a mismatch and name the x_lo*w_hi term of that k-block (a 1x1 conv: one tap)."""
+    import torch
+    from detectandtrack_b200 import _lib as L
+    from detectandtrack_b200.ops import conv as cv
+    layer = next(l for l in R50_FPN_3D if l[0] == 'res2 1x1 reduce')
+    Cin = layer[5]
+    g = torch.Generator(device='cuda').manual_seed(15)
+    run, ref_in = _step_inputs(layer, mode, g, operands='integer')
+    hi, lo = run['x'][..., :Cin], run['x'][..., Cin:]
+    bk = ref_in['bk']
+    lo2 = lo.clone()
+    lo2[..., bk:2 * bk] = 0
+    x = torch.cat([hi, lo, lo2], -1).contiguous()
+    orig = L.call
+
+    def lo_at_third_block(name, *a):
+        if name == 'dt_conv3d':
+            a[0]._obj.in_lo_off = 2 * Cin
+        return orig(name, *a)
+    monkeypatch.setattr(L, 'call', lo_at_third_block)
+    y = cv.conv3d(x, run['w'], run['k'], run['s'], run['p'], run['scale'], run['bias'], run['res'], run['rm'], run['relu'],
+                  dtype=run['dtype'])
+    monkeypatch.setattr(L, 'call', orig)
+    msg = _exact_mismatch(y, ref_in, layer[8], layer[9], 'wrong lo box')
+    assert msg is not None and 'x_lo*w_hi of tap (0, 0, 0), k-block 1 dropped' in msg, msg
 
 
 def test_step_convs_are_all_in_the_table(monkeypatch, record_property):

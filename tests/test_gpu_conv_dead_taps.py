@@ -7,7 +7,7 @@ import pytest
 from test_conv_dead_taps import EDGES, edge_plan
 from test_conv_plan import R50_FPN_3D, REDUCED, conv_args, plan
 from test_conv_reference import conv_ref
-from test_gpu_conv import _step_inputs
+from test_gpu_conv import _exact_mismatch, _integer_operands, _step_inputs, with_operands
 from test_gpu_train_grads import test_dgrad_of_every_step_layer_is_bf16_of_the_exact_sum as _dgrad_is_bf16_of_exact_sum
 from test_train_plan import D_REDUCED, ROWS, row_dplan
 
@@ -68,39 +68,48 @@ EDGE_TOL = {'bf16': 2e-4, 'tf32x3': 1e-4, 'bf16x3': 1e-4}
 EDGE_CASES = [(e, m) for e in EDGES for m in EDGE_MODES]
 
 
-@pytest.mark.parametrize('e,mode', EDGE_CASES, ids=['%s-%s' % (e[0], m) for e, m in EDGE_CASES])
-def test_edge_geometry_vs_fp64(e, mode):
+@with_operands('e,mode', EDGE_CASES, ['%s-%s' % (e[0], m) for e, m in EDGE_CASES])
+def test_edge_geometry_vs_fp64(e, mode, operands):
     """The edge geometries of the dead-tap rule (tests/test_conv_dead_taps.EDGES) against the fp64 tap-sum reference on
-    the values the kernel reads, with an affine, a bias of both signs and ReLU.  In bf16 (fp32 output) a tile without a
-    live group must give exactly relu(scale * 0 + bias)."""
+    the values the kernel reads (on integer operands: bit for bit), with an affine, a bias of both signs and ReLU.  In
+    bf16 (fp32 output) a tile without a live group must give exactly relu(scale * 0 + bias)."""
     import torch
     from detectandtrack_b200.ops import conv as cv
     name, N, T, H, W, Cin, Cout, k, s, p, out_t = e
     dt = cv.MODE_NAMES[mode]
     g = torch.Generator(device='cuda').manual_seed(zlib.crc32(('edge/%s/%s' % (name, mode)).encode()))
-    x = torch.randn((N, T, H, W, Cin), generator=g, device='cuda')
-    w = torch.randn((Cout, Cin) + k, generator=g, device='cuda') * (2.0 / (Cin * k[0] * k[1] * k[2])) ** 0.5
-    scale = torch.rand(Cout, generator=g, device='cuda') + 0.5
-    bias = torch.randn(Cout, generator=g, device='cuda') * 0.5
-    wp = cv.pack_weight(w, dt)
-    if dt in cv.SPLIT_MODES:
-        xd = cv.split_for(dt, x)
-        xr, wr = cv.join_split(xd), cv.join_split(wp)[:, :, :Cin]
+    frames = out_t if out_t[1] else None
+    if operands == 'integer':
+        xd, wp, scale, bias, _, ref = _integer_operands(g, (N, T, H, W), Cin, Cout, k, mode, True)
+        ref.update(res=[], res_mode=0, relu=True, kind={'bf16': 'f32', 'tf32x3': 'tf32 pair', 'bf16x3': 'bf16 pair'}[mode])
+        y = cv.conv3d(xd, wp, k, s, p, scale, bias, None, 0, True, out_f32=True if mode == 'bf16' else None, dtype=dt,
+                      out_frames=frames)
+        msg = _exact_mismatch(y, ref, s, p, '%s %s' % (name, mode), edge_plan(e, mode, out_f32=1), frames)
+        assert msg is None, msg
     else:
-        xd = x.bfloat16()
-        xr, wr = xd.float(), wp.float()[:, :, :Cin]
-    wr = wr.reshape(k + (Cout, Cin)).permute(3, 4, 0, 1, 2)
-    y = cv.conv3d(xd, wp, k, s, p, scale, bias, None, 0, True, out_f32=True if mode == 'bf16' else None, dtype=dt,
-                  out_frames=out_t if out_t[1] else None)
-    if dt in cv.SPLIT_MODES:
-        y = cv.join_split(y)
-    ref = conv_ref(xr, wr, s, p, scale, bias, relu=True)
-    if out_t[1]:
-        ref = ref[:, out_t[0]:out_t[0] + out_t[1]]
-    torch.cuda.synchronize()
-    assert y.shape == ref.shape
-    err = (y.double() - ref).abs().max().item()
-    assert err <= EDGE_TOL[mode] * ref.abs().max().item(), (name, mode, err)
+        x = torch.randn((N, T, H, W, Cin), generator=g, device='cuda')
+        w = torch.randn((Cout, Cin) + k, generator=g, device='cuda') * (2.0 / (Cin * k[0] * k[1] * k[2])) ** 0.5
+        scale = torch.rand(Cout, generator=g, device='cuda') + 0.5
+        bias = torch.randn(Cout, generator=g, device='cuda') * 0.5
+        wp = cv.pack_weight(w, dt)
+        if dt in cv.SPLIT_MODES:
+            xd = cv.split_for(dt, x)
+            xr, wr = cv.join_split(xd), cv.join_split(wp)[:, :, :Cin]
+        else:
+            xd = x.bfloat16()
+            xr, wr = xd.float(), wp.float()[:, :, :Cin]
+        wr = wr.reshape(k + (Cout, Cin)).permute(3, 4, 0, 1, 2)
+        y = cv.conv3d(xd, wp, k, s, p, scale, bias, None, 0, True, out_f32=True if mode == 'bf16' else None, dtype=dt,
+                      out_frames=frames)
+        if dt in cv.SPLIT_MODES:
+            y = cv.join_split(y)
+        ref = conv_ref(xr, wr, s, p, scale, bias, relu=True)
+        if out_t[1]:
+            ref = ref[:, out_t[0]:out_t[0] + out_t[1]]
+        torch.cuda.synchronize()
+        assert y.shape == ref.shape
+        err = (y.double() - ref).abs().max().item()
+        assert err <= EDGE_TOL[mode] * ref.abs().max().item(), (name, mode, err)
     if mode == 'bf16' and k[0] == 1 and p[0] > 0:      # the padded output frames read only zeros: no live group
         dead = torch.cat([y[:, :p[0]], y[:, -p[0]:]], 1)
         want = bias.clamp_min(0).expand_as(dead)

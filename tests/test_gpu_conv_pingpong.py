@@ -2,13 +2,14 @@
 over the other's ring stages, staging slots and residual chunks, so these cases aim at what that bookkeeping depends on:
 the number of tiles per CTA (odd, or one, where the second warpgroup has none), tiles without a live group next to live
 ones, live counts that differ from tile to tile, the residual and top-down rings, plain and [hi | lo] pair outputs.  Each
-is checked against the fp64 tap-sum reference on the values the kernel reads."""
+is checked against the fp64 tap-sum reference on the values the kernel reads, and on integer operands bit for bit."""
 import zlib
 
 import pytest
 
 from test_conv_plan import plan
 from test_conv_reference import conv_ref
+from test_gpu_conv import _exact_mismatch, _integer_operands, with_operands
 
 pytestmark = pytest.mark.gpu
 
@@ -61,8 +62,8 @@ CASES = [('one tile per CTA', 'bf16', 'plain'), ('one tile per CTA', 'bf16x3', '
          ('top-down', 'bf16', 'plain'), ('top-down', 'bf16x3', 'pair')]
 
 
-@pytest.mark.parametrize('kind,mode,output', CASES, ids=['%s-%s-%s' % c for c in CASES])
-def test_pingpong_vs_fp64(kind, mode, output):
+@with_operands('kind,mode,output', CASES, ['%s-%s-%s' % c for c in CASES])
+def test_pingpong_vs_fp64(kind, mode, output, operands):
     import torch
     from detectandtrack_b200.ops import conv as cv
     sms = _sms()
@@ -87,33 +88,43 @@ def test_pingpong_vs_fp64(kind, mode, output):
 
     g = torch.Generator(device='cuda').manual_seed(zlib.crc32(('pingpong/%s/%s/%s' % (kind, mode, output)).encode()))
     To, Ho, Wo = (T + 2 * p[0] - k[0]) // s[0] + 1, (H + 2 * p[1] - k[1]) // s[1] + 1, (W + 2 * p[2] - k[2]) // s[2] + 1
-    x = torch.randn((N, T, H, W, Cin), generator=g, device='cuda')
-    w = torch.randn((Cout, Cin) + k, generator=g, device='cuda') * (2.0 / (Cin * k[0] * k[1] * k[2])) ** 0.5
-    scale = torch.rand(Cout, generator=g, device='cuda') + 0.5
-    bias = torch.randn(Cout, generator=g, device='cuda') * 0.5
-    wp = cv.pack_weight(w, dt)
-    wr = (cv.join_split(wp) if split else wp.float())[:, :, :Cin].reshape(k + (Cout, Cin)).permute(3, 4, 0, 1, 2)
-    xd = cv.split_for(dt, x) if split else x.bfloat16()
-    xr = cv.join_split(xd) if split else xd.float()
-    res = resr = None
-    if rm:
-        r = torch.randn((N, To, Ho // rm, Wo // rm, Cout), generator=g, device='cuda')
-        res = cv.split_for(dt, r) if pair else (r if out_f32 else r.bfloat16())
-        resr = cv.join_split(res) if pair else res.float()
-    y = cv.conv3d(xd, wp, k, s, p, scale, bias, res, rm, True, out_f32=out_f32, dtype=dt, split_out=pair)
-    if pair:
-        y = cv.join_split(y)
-    ref = conv_ref(xr, wr, s, p, scale, bias, resr, rm, relu=True)
-    torch.cuda.synchronize()
-    assert y.shape == ref.shape
-    err = (y.double() - ref).abs()
-    den = ref.abs().max().item()
-    if y.dtype == torch.bfloat16:
-        bound = 2 ** -8 * ref.abs() + TOL[mode] * den
+    if operands == 'integer':
+        xd, wp, scale, bias, res, ref = _integer_operands(
+            g, (N, T, H, W), Cin, Cout, k, mode, True, (N, To, Ho // rm, Wo // rm, Cout) if rm else None,
+            torch.float32 if out_f32 else torch.bfloat16, pair)
+        ref.update(res_mode=rm, relu=True,
+                   kind=('%s pair' % mode[:4]) if pair else ('f32' if out_f32 else 'bf16'))
+        y = cv.conv3d(xd, wp, k, s, p, scale, bias, res, rm, True, out_f32=out_f32, dtype=dt, split_out=pair)
+        msg = _exact_mismatch(y, ref, s, p, '%s %s %s' % (kind, mode, output), o)
+        assert msg is None, msg
     else:
-        bound = torch.full_like(ref, TOL[mode] * den)
-    worst = (err / bound).max().item()
-    assert worst <= 1.0, (kind, mode, output, worst)
+        x = torch.randn((N, T, H, W, Cin), generator=g, device='cuda')
+        w = torch.randn((Cout, Cin) + k, generator=g, device='cuda') * (2.0 / (Cin * k[0] * k[1] * k[2])) ** 0.5
+        scale = torch.rand(Cout, generator=g, device='cuda') + 0.5
+        bias = torch.randn(Cout, generator=g, device='cuda') * 0.5
+        wp = cv.pack_weight(w, dt)
+        wr = (cv.join_split(wp) if split else wp.float())[:, :, :Cin].reshape(k + (Cout, Cin)).permute(3, 4, 0, 1, 2)
+        xd = cv.split_for(dt, x) if split else x.bfloat16()
+        xr = cv.join_split(xd) if split else xd.float()
+        res = resr = None
+        if rm:
+            r = torch.randn((N, To, Ho // rm, Wo // rm, Cout), generator=g, device='cuda')
+            res = cv.split_for(dt, r) if pair else (r if out_f32 else r.bfloat16())
+            resr = cv.join_split(res) if pair else res.float()
+        y = cv.conv3d(xd, wp, k, s, p, scale, bias, res, rm, True, out_f32=out_f32, dtype=dt, split_out=pair)
+        if pair:
+            y = cv.join_split(y)
+        ref = conv_ref(xr, wr, s, p, scale, bias, resr, rm, relu=True)
+        torch.cuda.synchronize()
+        assert y.shape == ref.shape
+        err = (y.double() - ref).abs()
+        den = ref.abs().max().item()
+        if y.dtype == torch.bfloat16:
+            bound = 2 ** -8 * ref.abs() + TOL[mode] * den
+        else:
+            bound = torch.full_like(ref, TOL[mode] * den)
+        worst = (err / bound).max().item()
+        assert worst <= 1.0, (kind, mode, output, worst)
     if kind == 'dead and live tiles' and output == 'f32':      # frames without a live group: exactly relu(bias)
         dead = torch.cat([y[:, :1], y[:, -1:]], 1)
         assert torch.equal(dead, bias.clamp_min(0).expand_as(dead))

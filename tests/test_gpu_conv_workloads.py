@@ -7,30 +7,32 @@ import pytest
 from test_conv_plan import step_plan
 from test_conv_plan_workloads import (CASES, STACKED_STRIDED, STACKED_STRIDED_REDUCED, TABLES, plan_key_v2, row_plan,
                                       table_keys)
-from test_gpu_conv import _check_step_case
+from test_gpu_conv import _check_step_case, with_operands
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize('wl,layer,mode', CASES, ids=['%s-%s-%s' % (w, l[0], m) for w, l, m in CASES])
-def test_workload_layer_over_three_waves_vs_fp64(wl, layer, mode, record_property):
+@with_operands('wl,layer,mode', CASES, ['%s-%s-%s' % (w, l[0], m) for w, l, m in CASES])
+def test_workload_layer_over_three_waves_vs_fp64(wl, layer, mode, operands, record_property):
     """Every (row, mode) of the three tables at its reduced shape (test_conv_plan_workloads: the step's plan and tile,
     three or more tiles per CTA, a ragged last wave, the step's partial tiles and skipped padding taps) with the engine's
     storage and epilogue, against the fp64 tap-sum reference on the values the kernel reads.  Among them: the strided
     3x3x3 branch2a of the R18 body on odd maps, the res5 RoI convs on stacks of 6 images x 3 frames of 7 x 7 with a ragged
     last stack, and the 3-D keypoint head on stacks of 3 images x 3 frames with a ragged last stack.  Bounds as in
-    test_gpu_conv.test_step_layer_over_three_waves_vs_fp64: bf16 outputs elementwise, the others _step_tol."""
+    test_gpu_conv.test_step_layer_over_three_waves_vs_fp64: bf16 outputs elementwise, the others _step_tol; integer
+    operands bit for bit."""
     _check_step_case(layer, mode, row_plan(wl, layer, mode, reduced=True), TABLES[wl][1], '%s/%s/%s' % (wl, layer[0], mode),
-                     record_property)
+                     record_property, operands)
 
 
-@pytest.mark.parametrize('mode', ('bf16', 'tf32', 'tf32x3', 'bf16x3'))
-def test_strided_conv_on_32_image_stacks_vs_fp64(mode, record_property):
+@with_operands('mode', ('bf16', 'tf32', 'tf32x3', 'bf16x3'), ('bf16', 'tf32', 'tf32x3', 'bf16x3'))
+def test_strided_conv_on_32_image_stacks_vs_fp64(mode, operands, record_property):
     """A strided 3x3 conv on 7 x 7 maps stacked 32 to an M tile (one output row of four columns each), 283 images: the
     strided activation box over stacked images, the live taps of each tile under stride, a last stack of 27 images."""
     o = step_plan(STACKED_STRIDED, mode, True, STACKED_STRIDED_REDUCED)
     assert (o.TB, o.TH, o.TW) == (32, 1, 4)
-    _check_step_case(STACKED_STRIDED, mode, o, STACKED_STRIDED_REDUCED, 'stacked-strided/%s' % mode, record_property)
+    _check_step_case(STACKED_STRIDED, mode, o, STACKED_STRIDED_REDUCED, 'stacked-strided/%s' % mode, record_property,
+                     operands)
 
 
 def test_workload_convs_are_all_in_the_tables(monkeypatch, record_property):

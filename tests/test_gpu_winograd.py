@@ -157,6 +157,41 @@ def test_wino_gemm_vs_fp64(cin):
     assert bool((err <= bound).all()), (err / a.clamp_min(1e-30)).max().item()
 
 
+@pytest.mark.parametrize('D', [1, 37, 104, 832])
+@pytest.mark.parametrize('cin', [256, 512])
+def test_wino_gemm_exact_on_integer_pairs(cin, D):
+    """M_xi = sum_c Vh Uh + Vl Uh + Vh Ul exactly, on independent integer hi / lo halves of V and U (the exact forward
+    check of test_conv_reference: every partial sum is an fp32 value while 3 a^2 Cin < 2^22), so a dropped, repeated or
+    misaddressed (k-block, product) shows.  D = 832 is the benchmarked 8 clips x 104 keypoint slots (G = 40768)."""
+    from test_conv_reference import EXACT_LIMIT, exact_bound, int_amplitude
+    cout = 512
+    G = D * NT * NT
+    a = int_amplitude(cin)
+    assert exact_bound(a, cin, True, 1.0, 0.0) < EXACT_LIMIT
+    g = torch.Generator(device='cuda').manual_seed(cin * 1000 + D)
+
+    def ints(shape):
+        return torch.randint(-a, a + 1, shape, generator=g, device='cuda').double()
+    vh, vl, uh, ul = ints((16, G, cin)), ints((16, G, cin)), ints((16, cout, cin)), ints((16, cout, cin))
+    v = torch.cat([vh, vl], -1).to(torch.bfloat16).contiguous()
+    u = torch.cat([uh, ul], -1).to(torch.bfloat16).contiguous()
+    m = torch.full((16, G, cout), float('nan'), dtype=torch.float32, device='cuda')
+    cv.wino_gemm(v, u, m, G)
+    terms = {'V_hi*U_hi': (vh, uh), 'V_lo*U_hi': (vl, uh), 'V_hi*U_lo': (vh, ul)}
+    ref = sum(torch.bmm(p, q.transpose(1, 2)) for p, q in terms.values())
+    assert float((torch.bmm(vl, ul.transpose(1, 2)) != 0).double().mean()) > 0.5      # lo*lo added would show
+    bad = m.double() != ref
+    if bool(bad.any()):
+        xi, gi, co = [int(i) for i in torch.unravel_index(bad.view(-1).nonzero()[0, 0], bad.shape)]
+        diff = float(m[xi, gi, co]) - float(ref[xi, gi, co])
+        hits = ['%s of k-block %d %s' % (n, kb, 'dropped' if c == -diff else 'added twice')
+                for n, (p, q) in terms.items() for kb in range(cin // 64)
+                for c in [float((p[xi, gi, kb * 64:(kb + 1) * 64] * q[xi, co, kb * 64:(kb + 1) * 64]).sum())]
+                if c != 0 and abs(c) == abs(diff)]
+        pytest.fail('%d wrong entries of M; first (component %d, tile %d, Cout %d): difference %r; equals a single term: %s'
+                    % (int(bad.sum()), xi, gi, co, diff, '; '.join(hits) or 'none'))
+
+
 def _layer_inputs(D, cin, cout, seed):
     rng = np.random.RandomState(seed)
     xs = np.abs(rng.randn(D, 1, S, S, cin)).astype(np.float32)         # post-ReLU activations
