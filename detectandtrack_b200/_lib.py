@@ -45,14 +45,11 @@ SIGNATURES = {
     'dt_spatial_mean': [_p, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p],
     'dt_time_mean': [_p, _i, _i, C.c_longlong, _i, _i, _i, _i, _i, _p, _i, _p],
     'dt_fold_tube_heads': [_p, _i, _i, _i, _i, _p, _p, _p],
-    'dt_to_planes': [_p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _p],
-    'dt_wgrad': [_p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _p],
     'dt_wgrad_nhwc': [_p, _i, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _p],
     'dt_bwd_pointwise': [_p, _p, _p, _p, C.c_longlong, _i, _p, _p],
     'dt_bwd_pointwise2': [_p, _p, _p, _p, C.c_longlong, _i, _p, _p, _p, _p],
     'dt_upsample_add_bwd': [_p, _p, _i, _i, _i, _i, _p, _p],
     'dt_scatter_stride2': [_p, _i, _i, _i, _i, _i, _i, _p, _p],
-    'dt_sgd_update': [_p, _p, _p, _i, _i, _i, _f, _f, _f, _f, _p, _p, _p],
     'dt_sgd_update_multi': [_p, _p, _i, _i, _f, _f, _f, _f, _p],
     'dt_bias_grad': [_p, C.c_longlong, _i, _i, _p, _p],
     'dt_rpn_loss_grad': [_p, _i, _p, _p, _p, _p, C.c_longlong, _i, _f, _f, _f, _p, _i, _p, _p],
@@ -71,7 +68,7 @@ SIGNATURES = {
 # host-only helpers: no device work, usable without a GPU (dt_wgrad_nhwc_plan returns 0 or an error code like the rest).
 # dt_prep_batch does launch a kernel; it is listed here rather than in SIGNATURES because its argument-error cases live
 # in tests/test_train_augment.py, one per host check, not in the single-case table of tests/test_capi_errors.py.
-HOST_FUNCS = {'dt_planes_ld': ([_i, _i, _i, _i], C.c_int), 'dt_jpeg_available': ([], C.c_int),
+HOST_FUNCS = {'dt_jpeg_available': ([], C.c_int),
               'dt_wgrad_nhwc_plan': ([_i] * 15 + [C.c_void_p], C.c_int),
               'dt_prep_batch': ([C.POINTER(_p), C.POINTER(_i), C.POINTER(_i), C.POINTER(C.c_double), C.POINTER(_i), C.POINTER(_i),
                                  C.POINTER(_i), _i, _i, C.POINTER(_f), _i, _i, _i, _i, _i, _i, _i, _p, _p], C.c_int),

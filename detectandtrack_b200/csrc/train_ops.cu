@@ -1,55 +1,42 @@
 // Training-step kernels of the data-parallel path (BASELINE.json configs[4]; the reference builds these with
 // model.AddGradientOperators + add_parameter_update_ops, lib/modeling/model_builder.py:908-985):
 //
-//   dt_wgrad            Conv / ConvNd filter gradient on the tensor cores (wgmma):
+//   dt_wgrad_nhwc       Conv / ConvNd / FC filter gradient on the tensor cores (wgmma):
 //                         dW[tap][co][ci] = sum over positions of gz[pos, co] * x[pos @ tap, ci]
-//                       a GEMM whose K axis is the position axis.  Both operands are read from CHANNEL-MAJOR PLANES
-//                       ([N, T, C, plane], plane = the zero-bordered (H+2p) x (W+2p) map flattened), so a position run is
-//                       contiguous (a K-major operand for wgmma, staged by TMA with the 128B swizzle) and a filter ROW
-//                       offset (kh) is a constant offset along the flattened plane (rows are padded to a multiple of 8
-//                       positions, so the offset keeps TMA's 16-byte alignment of the innermost coordinate; the physical
-//                       zero border supplies the padding, TMA's out-of-bounds zero fill the plane ends and the temporal
-//                       padding).  A +-1 COLUMN offset (kw) would break that alignment, so the input planes are stored kW
-//                       times, copy kw pre-shifted by kw - pW positions (dt_to_planes wshift).  Split-K over positions
-//                       across CTAs, fp32 partial sums reduced into dW with vector red.global.
-//   dt_to_planes        NDHWC activation / gradient -> those planes (tiled transpose through shared memory, optional
-//                       spatial subsampling for the strided 1x1 convs).
+//                       a GEMM whose K axis is the position axis, both operands read straight from the NDHWC tensors by
+//                       5-D TMA boxes of 64 positions (MN-major wgmma operands; the tap is a coordinate shift of the input
+//                       box, TMA's zero fill the padding).  Split-K over positions across CTAs, fp32 partial sums reduced
+//                       into dW with vector red.global.
 //   dt_bwd_pointwise    the elementwise part of a block's backward: gz = (g1 + g2) * [y > 0] * scale[c]
 //                       (Relu / Sum / AffineChannelNd gradients, lib/ops/affine_channel_nd_op.cu:73-92: dX = dY * scale;
 //                       the affine parameters themselves are frozen in Detectron-style fine-tuning)
 //   dt_upsample_add_bwd FPN top-down join backward (lib/modeling/FPN3D.py:186-222): the coarser level receives the 2x2 sum
 //   dt_scatter_stride2  dgrad of a stride-2 pointwise conv: values land on the even positions of a zeroed map
-//   dt_sgd_update       MomentumSGDUpdate with weight decay (model_builder.py:954-985) on fp32 master weights kept in the
-//                       packed [tap][Cout][Cin] order, re-emitting the bf16 forward weights and the (flipped, transposed)
-//                       bf16 dgrad weights in the same pass
+//   dt_sgd_update_multi MomentumSGDUpdate with weight decay (model_builder.py:954-985) of every parameter tensor in one
+//                       launch, on fp32 master weights kept in the packed [tap][Cout][Cin] order, re-emitting the bf16
+//                       forward weights and the (flipped, transposed) bf16 dgrad weights in the same pass
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "../../include/dt_b200.h"
 #include <cuda_bf16.h>
-#include <stdlib.h>
 
 namespace dt {
 
 using namespace tc;
 
 // ------------------------------------------------------------------------------------------------ wgrad
-struct WgradParams {
-  int Cout, Cin, taps;
-  int kT, kH, kW, pT, pH, pW;
-  int Wp;                 // row length of the padded plane (W + 2*pW rounded up to 8)
-  int T, N;               // frames, images
-  int kchunks;            // 64-position chunks per plane
-  int tiles_m, tiles_n, ksplit;
-  float* dW;              // [taps][Cout][Cin] fp32, accumulated into (caller zeroes)
-};
-
+// The GEMM read STRAIGHT from the NDHWC tensors: a TMA box (64 channels = 128 B, TW, TH, TT, TB) of 64 positions lands in
+// shared memory as 64 rows of 128 bytes — positions down the rows, 64 channels along each swizzled row.  Read as an
+// MN-MAJOR wgmma operand (the transpose flags of the instruction) with K = the position axis: 8 positions x 128 B per
+// swizzle atom, 1024 B between 8-position groups.  The filter tap is a coordinate shift of the input box (TMA zero fill =
+// the conv's padding), exactly as in the forward kernel.
 constexpr int WG_THREADS = 384;       // warp 0 TMA producer (warps 1-3 idle), warps 4-11 two consumer warpgroups
 constexpr int WG_CONSUMER_WARPS = 8;
 constexpr int WG_STAGES = 4;
 
-// Consumers of both wgrad kernels: warpgroup g accumulates rows (output channels) 64g .. 64g+63 of the 128-row tile in
-// registers (fragment layout: wgmma.cuh) and adds them into dW with red.global.  Cin is even, so a thread's column pair
-// is either wholly inside the filter or wholly outside.
+// Consumers: warpgroup g accumulates rows (output channels) 64g .. 64g+63 of the 128-row tile in registers (fragment
+// layout: wgmma.cuh) and adds them into dW with red.global.  Cin is even, so a thread's column pair is either wholly
+// inside the filter or wholly outside.
 template <int NB>
 __device__ __forceinline__ void wgrad_red(const float (&acc)[NB], float* dW, int Cout, int Cin, int tap, int row_base, int col_base) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -66,115 +53,6 @@ __device__ __forceinline__ void wgrad_red(const float (&acc)[NB], float* dW, int
   }
 }
 
-template <int BN>
-__global__ void __launch_bounds__(WG_THREADS, 1)
-wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmX, const WgradParams p) {
-  constexpr int A_BYTES = 128 * 128, B_BYTES = BN * 128, ST_BYTES = A_BYTES + B_BYTES;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * ST_BYTES);
-  uint64_t* empty = full + WG_STAGES;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    if ((smem_u32(smem) & 1023u) != 0) __trap();
-    prefetch_tmap(&tmG); prefetch_tmap(&tmX);
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], WG_CONSUMER_WARPS); }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  // work item: (tap, m tile, n tile, k split)
-  int w = blockIdx.x;
-  const int ks = w % p.ksplit; w /= p.ksplit;
-  const int nt = w % p.tiles_n; w /= p.tiles_n;
-  const int mt = w % p.tiles_m;
-  const int tap = w / p.tiles_m;
-  const int kw = tap % p.kW, kh = (tap / p.kW) % p.kH, kt = tap / (p.kW * p.kH);
-  const int shift = (kh - p.pH) * p.Wp;          // filter-row offset along the flattened padded plane (multiple of 8: 16-byte
-                                                 // aligned TMA coordinate); the column offset selects the pre-shifted copy kw
-  const int dt_ = kt - p.pT;
-  // k-blocks = (image, frame, chunk) triples; frames whose tap-shifted source frame is outside the clip contribute zero
-  // (temporal zero padding) and are skipped by producer and consumers alike
-  const long long total = (long long)p.N * p.T * p.kchunks;
-  const long long k0 = total * ks / p.ksplit, k1 = total * (ks + 1) / p.ksplit;
-
-  if (warp == 0) {
-    int stage = 0; uint32_t phase = 0;
-    long long r = k0 / p.kchunks;
-    int chunk = (int)(k0 - r * p.kchunks);
-    int t = (int)(r % p.T), n = (int)(r / p.T);
-    for (long long kb = k0; kb < k1; ++kb) {
-      const int ts = t + dt_;
-      if (ts >= 0 && ts < p.T) {
-        mbar_wait(&empty[stage], phase ^ 1);
-        if (elect_one()) {
-          const uint32_t dst = smem_u32(smem) + stage * ST_BYTES;
-          const uint32_t bar = smem_u32(&full[stage]);
-          mbar_expect_tx_u(bar, (uint32_t)ST_BYTES);
-          // A: gz planes, box (64 positions, 128 channels); B: x planes at the tap-shifted position / frame
-          asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(&tmG)), "r"(bar), "r"(chunk * 64), "r"(mt * 128), "r"(t), "r"(n) : "memory");
-          asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-                       ::"r"(dst + A_BYTES), "l"(reinterpret_cast<uint64_t>(&tmX)), "r"(bar), "r"(chunk * 64 + shift), "r"(nt * BN), "r"(ts), "r"(n), "r"(kw) : "memory");
-        }
-        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (++chunk == p.kchunks) { chunk = 0; if (++t == p.T) { t = 0; ++n; } }
-    }
-  } else if (warp >= 4) {
-    const uint32_t a_base = smem_u32(smem) + (uint32_t)((warp - 4) >> 2) * (64u * 128u);   // this warpgroup's 64 rows
-    int stage = 0; uint32_t phase = 0;
-    long long r = k0 / p.kchunks;
-    int chunk = (int)(k0 - r * p.kchunks);
-    int t = (int)(r % p.T);
-    long long kb = k0;
-    // walk to the next live k-block (the wgmmas below then sit in the loop body, not under a branch)
-    auto skip_dead = [&]() {
-      while (kb < k1 && (t + dt_ < 0 || t + dt_ >= p.T)) { ++kb; if (++chunk == p.kchunks) { chunk = 0; if (++t == p.T) t = 0; } }
-    };
-    skip_dead();
-    const bool any = kb < k1;          // a range made only of temporally padded frames accumulates nothing
-    float acc[BN / 2];
-    int prev = -1;
-    uint32_t first = 1;
-    while (kb < k1) {
-      mbar_wait(&full[stage], phase);
-      const uint64_t adesc = make_sw128_desc(a_base + stage * ST_BYTES);
-      const uint64_t bdesc = make_sw128_desc(smem_u32(smem) + stage * ST_BYTES + A_BYTES);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma<BN, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (first && k == 0) ? 0u : 1u);
-      wgmma_commit();
-      wgmma_wait<1>();
-      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
-      prev = stage;
-      first = 0;
-      if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-      ++kb; if (++chunk == p.kchunks) { chunk = 0; if (++t == p.T) t = 0; }
-      skip_dead();
-    }
-    wgmma_wait<0>();
-    if (any) wgrad_red<BN / 2>(acc, p.dW, p.Cout, p.Cin, tap, mt * 128, nt * BN);
-  }
-}
-
-template <int BN>
-static int launch_wgrad(const CUtensorMap& tmG, const CUtensorMap& tmX, const WgradParams& p, cudaStream_t stream) {
-  constexpr int smem = WG_STAGES * (128 * 128 + BN * 128) + 256;
-  static DynSmemGrant grant;
-  DT_CHECK_CUDA(grant_dyn_smem(wgrad_kernel<BN>, smem, &grant));
-  const long long grid = (long long)p.taps * p.tiles_m * p.tiles_n * p.ksplit;
-  DT_CHECK_ARG(grid < (1ll << 31), "dt_wgrad: grid too large");
-  wgrad_kernel<BN><<<(unsigned)grid, WG_THREADS, smem, stream>>>(tmG, tmX, p);
-  DT_CHECK_LAUNCH();
-  return 0;
-}
-
-// ------------------------------------------------------------------------------------------------ wgrad, NDHWC operands
-// The same GEMM read STRAIGHT from the NDHWC tensors (no channel-major copies): a TMA box (64 channels = 128 B, TW, TH, TT, TB)
-// of 64 positions lands in shared memory as 64 rows of 128 bytes — positions down the rows, 64 channels along each swizzled
-// row.  Read as an MN-MAJOR wgmma operand (the transpose flags of the instruction) with K = the position axis: 8 positions
-// x 128 B per swizzle atom, 1024 B between 8-position groups.  The filter tap is a coordinate shift of the input box (TMA
-// zero fill = the conv's padding), exactly as in the forward kernel, so kw needs no pre-shifted copies.
 struct WgradNParams {
   int Cout, Cin, taps;
   int kT, kH, kW, pT, pH, pW;
@@ -300,54 +178,6 @@ static int launch_wgrad_nhwc(const CUtensorMap& tmG, const CUtensorMap& tmX, con
   return 0;
 }
 
-// ------------------------------------------------------------------------------------------------ planes
-// x [N*T frames, H, W, ldx] (first C channels) -> planes [copies][N*T, C, Pld]: plane position ((h / sh) + pH) * Wp + (w / sw) + pW
-// for h % sh == 0, w % sw == 0; border and row tail zero.  Copy j holds the plane shifted by wshift0 + j columns (column c of
-// the copy = pixel column c + shift; the wgrad input operand: one copy per filter column).  Tile: 64 plane positions (+ the
-// shift halo) x 64 channels staged ONCE in shared memory, every copy written from it.
-constexpr int TP_HALO = 3;
-__global__ void __launch_bounds__(256)
-to_planes_kernel(const __nv_bfloat16* __restrict__ x, int F, int H, int W, int C, int ldx, int sh, int sw, int pH, int pW,
-                 int wshift0, int ncopies, int Ho, int Wo, int Pld, long long copy_stride, __nv_bfloat16* __restrict__ out) {
-  __shared__ __nv_bfloat16 tile[64 + 2 * TP_HALO][66];
-  const int Wp = (Wo + 2 * pW + 7) / 8 * 8;
-  const int plane = (Ho + 2 * pH) * Wp;
-  const int p0 = blockIdx.x * 64, c0 = blockIdx.y * 64, f = blockIdx.z;
-  // load the UNSHIFTED plane positions p0 - HALO .. p0 + 64 + HALO: thread -> (position, 16-byte channel group)
-  for (int i = threadIdx.x; i < (64 + 2 * TP_HALO) * 8; i += blockDim.x) {
-    const int pp = i >> 3, cg = (i & 7) * 8;
-    const int pos = p0 - TP_HALO + pp;
-    uint4 v = make_uint4(0, 0, 0, 0);
-    if (pos >= 0 && pos < plane && c0 + cg < C) {
-      const int hp = pos / Wp, wp = pos - hp * Wp;
-      const int ho = hp - pH, wo = wp - pW;
-      if (ho >= 0 && ho < Ho && wo >= 0 && wo < Wo)
-        v = *reinterpret_cast<const uint4*>(x + (((size_t)f * H + (size_t)ho * sh) * W + (size_t)wo * sw) * ldx + c0 + cg);
-    }
-    const __nv_bfloat16* e = reinterpret_cast<const __nv_bfloat16*>(&v);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) tile[pp][cg + j] = e[j];
-  }
-  __syncthreads();
-  // store: thread -> (copy, channel, 8 consecutive positions).  Copy with shift d at column wp shows the pixel of column
-  // wp + d, i.e. the staged position + d, unless that column falls outside the padded row (then zero: rows do not wrap).
-  const __nv_bfloat16 zero = __float2bfloat16_rn(0.f);
-  for (int i = threadIdx.x; i < ncopies * 64 * 8; i += blockDim.x) {
-    const int cp = i / 512, rem = i - cp * 512;
-    const int cc = rem >> 3, pg = (rem & 7) * 8;
-    if (c0 + cc >= C || p0 + pg >= Pld) continue;
-    const int d = wshift0 + cp;
-    __align__(16) __nv_bfloat16 v[8];
-    const int hp0 = (p0 + pg) / Wp, wp0 = (p0 + pg) - hp0 * Wp;       // Wp % 8 == 0: the 8 positions share a row
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int wsrc = wp0 + j + d;
-      v[j] = (wsrc >= 0 && wsrc < Wp) ? tile[pg + j + d + TP_HALO][cc] : zero;
-    }
-    *reinterpret_cast<uint4*>(out + (size_t)cp * copy_stride + ((size_t)f * C + c0 + cc) * Pld + p0 + pg) = *reinterpret_cast<const uint4*>(v);
-  }
-}
-
 // ------------------------------------------------------------------------------------------------ pointwise backward
 __global__ void bwd_pointwise_kernel(const __nv_bfloat16* __restrict__ g1, const __nv_bfloat16* __restrict__ g2,
                                      const __nv_bfloat16* __restrict__ y, const float* __restrict__ scale, long long rows,
@@ -457,40 +287,12 @@ __global__ void embed_frame_kernel(const uint4* __restrict__ src, long long per_
 
 // ------------------------------------------------------------------------------------------------ SGD
 // Caffe2 MomentumSGDUpdate (non-Nesterov): g' = lr * (grad_scale * g + wd * w) + momentum * m;  m = g';  w -= g'
-// w / g / m [taps][Cout][Cin] fp32.  Re-emits wf [taps][Cout][Cin] bf16 (forward operand) and wd_ [taps][Cin][Cout] bf16
+// w / g / m [taps][Cout][Cin] fp32.  Re-emits wf [taps][Cout][Cin] bf16 (forward operand) and wdg [taps][Cin][Cout] bf16
 // with the taps FLIPPED (dgrad of a stride-1 "same" conv is the conv of the gradient with the flipped, transposed filter).
-// grid (ci tiles of 32, co tiles of 32, taps), block (32, 8): coalesced fp32 reads / writes along Cin, the transposed dgrad
-// filter written through a shared-memory tile so that its stores are coalesced along Cout as well
-__global__ void __launch_bounds__(256)
-sgd_update_kernel(float* __restrict__ w, const float* __restrict__ g, float* __restrict__ m, int taps, int Cout, int Cin, float lr,
-                  float momentum, float wd, float grad_scale, __nv_bfloat16* __restrict__ wf, __nv_bfloat16* __restrict__ wdg) {
-  __shared__ float tile[32][33];
-  const int tap = blockIdx.z, co0 = blockIdx.y * 32, ci0 = blockIdx.x * 32;
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  for (int r = ty; r < 32; r += 8) {
-    const int co = co0 + r, ci = ci0 + tx;
-    float nw = 0.f;
-    if (co < Cout && ci < Cin) {
-      const size_t i = ((size_t)tap * Cout + co) * Cin + ci;
-      const float wi = w[i];
-      const float adj = lr * (grad_scale * g[i] + wd * wi) + momentum * m[i];
-      m[i] = adj;
-      nw = wi - adj;
-      w[i] = nw;
-      if (wf) wf[i] = __float2bfloat16_rn(nw);
-    }
-    tile[r][tx] = nw;
-  }
-  if (!wdg) return;
-  __syncthreads();
-  for (int r = ty; r < 32; r += 8) {
-    const int ci = ci0 + r, co = co0 + tx;
-    if (ci < Cin && co < Cout) wdg[((size_t)(taps - 1 - tap) * Cin + ci) * Cout + co] = __float2bfloat16_rn(tile[tx][r]);
-  }
-}
-
 // Every parameter tensor of the model in ONE launch: a table of items (device memory, built once by the trainer) and the
-// exclusive prefix of their 32x32 tile counts; a block finds its item by binary search and runs the same tile update.
+// exclusive prefix of their 32x32 tile counts; a block finds its item by binary search and updates one (tap, 32 Cout,
+// 32 Cin) tile with 256 threads as (32, 8): coalesced fp32 reads / writes along Cin, the transposed dgrad filter written
+// through a shared-memory tile so that its stores are coalesced along Cout as well.
 struct SgdItem {
   float* w; const float* g; float* m; __nv_bfloat16* wf; __nv_bfloat16* wdg;
   int taps, Cout, Cin, tiles_ci, tiles_co;
@@ -862,67 +664,6 @@ static int grid_for(long long total, int block) {
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
-extern "C" int dt_planes_ld(int Ho, int Wo, int pH, int pW) { return (Ho + 2 * pH) * ((Wo + 2 * pW + 7) / 8 * 8); }
-
-extern "C" int dt_to_planes(const void* x, int F, int H, int W, int C, int ldx, int sh, int sw, int pH, int pW, int wshift,
-                            int ncopies, void* out, void* stream) {
-  DT_CHECK_ARG(F >= 0 && H >= 1 && W >= 1 && C >= 8 && C % 8 == 0 && ldx >= C && ldx % 8 == 0 && sh >= 1 && sw >= 1 && pH >= 0 && pW >= 0,
-               "dt_to_planes: bad shape F=%d H=%d W=%d C=%d ldx=%d", F, H, W, C, ldx);
-  DT_CHECK_ARG(ncopies >= 1 && wshift >= -pW && wshift + ncopies - 1 <= pW && pW <= TP_HALO,
-               "dt_to_planes: shifts %d..%d outside [-%d, %d] (pW <= %d)", wshift, wshift + ncopies - 1, pW, pW, TP_HALO);
-  if (F == 0) return 0;
-  DT_CHECK_ARG(x && out, "dt_to_planes: null pointer");
-  const int Ho = (H + sh - 1) / sh, Wo = (W + sw - 1) / sw;
-  const int Pld = dt_planes_ld(Ho, Wo, pH, pW);
-  dim3 grid((Pld + 63) / 64, (C + 63) / 64, F);
-  to_planes_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, F, H, W, C, ldx, sh, sw, pH, pW, wshift, ncopies, Ho, Wo, Pld,
-                                                           (long long)F * C * Pld, (__nv_bfloat16*)out);
-  DT_CHECK_LAUNCH();
-  return 0;
-}
-
-extern "C" int dt_wgrad(const void* gz_planes, const void* x_planes, int N, int T, int Ho, int Wo, int Cout, int Cin, int kT, int kH,
-                        int kW, float* dW, void* stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
-  DT_CHECK_ARG(N >= 1 && T >= 1 && Ho >= 1 && Wo >= 1 && Cout >= 1 && Cin >= 8 && Cin % 8 == 0 && kT >= 1 && kH >= 1 && kW >= 1 &&
-                   (kT & 1) && (kH & 1) && (kW & 1),
-               "dt_wgrad: bad shape N=%d T=%d %dx%d Cout=%d Cin=%d k=%dx%dx%d (odd 'same' kernels, Cin %% 8 == 0)", N, T, Ho, Wo, Cout, Cin, kT, kH, kW);
-  DT_CHECK_ARG(gz_planes && x_planes && dW, "dt_wgrad: null pointer");
-  DT_CHECK_ARG(((uintptr_t)dW & 7) == 0, "dt_wgrad: dW must be 8-byte aligned (red.global.add.v2.f32)");
-  const int pT = kT / 2, pH = kH / 2, pW = kW / 2;
-  const int Pld = dt_planes_ld(Ho, Wo, pH, pW);
-  const int Wp = (Wo + 2 * pW + 7) / 8 * 8, plane = Pld;
-  WgradParams p;
-  memset(&p, 0, sizeof(p));
-  p.Cout = Cout; p.Cin = Cin; p.taps = kT * kH * kW; p.kT = kT; p.kH = kH; p.kW = kW; p.pT = pT; p.pH = pH; p.pW = pW;
-  p.Wp = Wp; p.T = T; p.N = N; p.kchunks = cdiv(plane, 64); p.dW = dW;
-  const int BN = Cin > 64 ? 128 : 64;      // 128 x BN fp32 accumulators live in the registers of two warpgroups
-  p.tiles_m = cdiv(Cout, 128); p.tiles_n = cdiv(Cin, BN);
-  const long long units = (long long)p.taps * p.tiles_m * p.tiles_n;
-  const long long kblocks = (long long)N * T * p.kchunks;
-  long long ksplit = (num_sms() * 3ll + units - 1) / units;               // ~3 waves of CTAs
-  if (ksplit > kblocks / 4) ksplit = kblocks / 4;
-  if (ksplit < 1) ksplit = 1;
-  p.ksplit = (int)ksplit;
-  CUtensorMap tmG, tmX;
-  {
-    uint64_t d[4] = {(uint64_t)plane, (uint64_t)Cout, (uint64_t)T, (uint64_t)N};
-    uint64_t s[3] = {(uint64_t)Pld * 2, (uint64_t)Pld * 2 * Cout, (uint64_t)Pld * 2 * Cout * T};
-    uint32_t b[4] = {64, 128, 1, 1}, e[4] = {1, 1, 1, 1};
-    if (encode_map(&tmG, 0, 4, gz_planes, d, s, b, e)) return 1;
-  }
-  {   // x planes: kW pre-shifted copies [kW][N*T, Cin, Pld]
-    uint64_t d[5] = {(uint64_t)plane, (uint64_t)Cin, (uint64_t)T, (uint64_t)N, (uint64_t)kW};
-    uint64_t s[4] = {(uint64_t)Pld * 2, (uint64_t)Pld * 2 * Cin, (uint64_t)Pld * 2 * Cin * T, (uint64_t)Pld * 2 * Cin * T * N};
-    uint32_t b[5] = {64, (uint32_t)BN, 1, 1, 1}, e[5] = {1, 1, 1, 1, 1};
-    if (encode_map(&tmX, 0, 5, x_planes, d, s, b, e)) return 1;
-  }
-  switch (BN) {
-    case 128: return launch_wgrad<128>(tmG, tmX, p, stream);
-    default: return launch_wgrad<64>(tmG, tmX, p, stream);
-  }
-}
-
 // What dt_wgrad_nhwc launches, derived in one place for the launcher and dt_wgrad_nhwc_plan (the plan is what runs):
 // argument checks, the 64-position tile, BN, the tile counts, the K split, the grid and the dynamic shared memory.
 static int wgrad_nhwc_geom(int ld_g, int ld_x, int N, int T, int Ho, int Wo, int Hi, int Wi, int Cout, int Cin, int kT, int kH, int kW,
@@ -956,11 +697,9 @@ static int wgrad_nhwc_geom(int ld_g, int ld_x, int N, int T, int Ho, int Wo, int
   const long long units = (long long)p.taps * p.tiles_m * p.tiles_n;
   const long long kblocks = (long long)p.nW * p.nH * p.nT * p.nN;
   // K split: every CTA adds its 128 x BN partial tile into dW with red.global, so the split count is also the atomic
-  // traffic multiplier.  DT_WGRAD_WAVES overrides the wave count (tuning knob of tools/bench_wgrad.py).
-  // Pointwise layers use ONE wave of CTAs (a 1x1 filter has few (tap, tile) units, so more waves mean many partial tiles
-  // added per output tile), multi-tap layers two.
-  static const int waves_env = [] { const char* e = getenv("DT_WGRAD_WAVES"); const int v = e ? atoi(e) : 0; return v >= 1 && v <= 16 ? v : 0; }();
-  const int waves = waves_env ? waves_env : (p.taps == 1 ? 1 : 2);
+  // traffic multiplier.  Pointwise layers use ONE wave of CTAs (a 1x1 filter has few (tap, tile) units, so more waves
+  // mean many partial tiles added per output tile), multi-tap layers two.
+  const int waves = p.taps == 1 ? 1 : 2;
   long long ksplit = ((long long)num_sms() * waves + units - 1) / units;
   if (ksplit > kblocks / 4) ksplit = kblocks / 4;
   if (ksplit < 1) ksplit = 1;
@@ -1062,17 +801,6 @@ extern "C" int dt_embed_frame(const void* src, int B, int T, long long frame_ele
   DT_CHECK_ARG(src && out, "dt_embed_frame: null pointer");
   DT_CHECK_ARG(aligned16(src) && aligned16(out), "dt_embed_frame: src / out must be 16-byte aligned");
   embed_frame_kernel<<<grid_for((long long)B * T * (frame_elems / 8), 256), 256, 0, (cudaStream_t)stream>>>((const uint4*)src, frame_elems / 8, B, T, c, (uint4*)out);
-  DT_CHECK_LAUNCH();
-  return 0;
-}
-
-extern "C" int dt_sgd_update(float* w, const float* g, float* m, int taps, int Cout, int Cin, float lr, float momentum, float wd,
-                             float grad_scale, void* w_fwd_bf16, void* w_dgrad_bf16, void* stream) {
-  DT_CHECK_ARG(taps >= 1 && taps <= 65535 && Cout >= 1 && Cin >= 1 && (Cout + 31) / 32 <= 65535, "dt_sgd_update: bad shape");
-  DT_CHECK_ARG(w && g && m, "dt_sgd_update: null pointer");
-  dim3 grid((Cin + 31) / 32, (Cout + 31) / 32, taps);
-  sgd_update_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(w, g, m, taps, Cout, Cin, lr, momentum, wd, grad_scale,
-                                                            (__nv_bfloat16*)w_fwd_bf16, (__nv_bfloat16*)w_dgrad_bf16);
   DT_CHECK_LAUNCH();
   return 0;
 }

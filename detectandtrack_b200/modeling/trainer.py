@@ -6,7 +6,7 @@ Implemented graph: the reference's RPN training model (``MODEL.TYPE rpn``, model
 frozen (freeze_at=2, ResNet3D.py:273-274; AffineChannel parameters frozen everywhere), res3..res5 + FPN + RPN heads
 trained: forward in bf16 (fp32 accumulate), backward =
     dgrad   dt_conv3d with the flipped / transposed filter (+ dt_scatter_stride2 for the stride-2 1x1 convs)
-    wgrad   dt_wgrad on channel-major planes (wgmma, split-K)
+    wgrad   dt_wgrad_nhwc straight from the NDHWC gradient and saved input (wgmma, split-K)
     joins   dt_bwd_pointwise (Relu / Sum / AffineChannelNd gradients), dt_upsample_add_bwd (FPN top-down), dt_bias_grad
     losses  dt_rpn_loss_grad per level (SigmoidCrossEntropyLoss + SmoothL1Loss)
 then a bucketed gradient SUM all-reduce over NCCL issued per bucket as soon as its filter gradients are enqueued
@@ -22,8 +22,6 @@ and all on the device,
                upsampling (dt_kps_loss_grad)
     backward   the FC / conv layers through the same dgrad / wgrad kernels (an FC is a 1x1 conv over the RoI axis),
                dt_roi_align_bwd into fp32 per-level accumulators that join the RPN's feature gradients."""
-import os
-
 import numpy as np
 
 from .. import _lib as L
@@ -31,9 +29,6 @@ from ..ops import conv as cv, dense_ops, train_ops as to, rpn_ops, box_ops, targ
 from . import params as P
 from .engine import DetectionEngine, im_scale_and_size, padded_blob_size
 from .generate_anchors import generate_anchors
-
-
-WGRAD_PLANES = os.environ.get('DT_WGRAD_PLANES', '0') == '1'
 
 
 def plan_buckets(counts, nbuckets):
@@ -121,18 +116,11 @@ class TrainConv(object):
         return cv.conv3d(x, self.w_fwd, self.k, self.stride, self.pad, self.scale, self.shift if self.bias is None else self.bias,
                          residual, res_mode, self.relu, out_f32=out_f32, dtype=cv.BF16, out=out, time_major=time_major)
 
-    def backward(self, gz, x, x_planes=None, need_dx=True):
+    def backward(self, gz, x, need_dx=True):
         """gz: gradient wrt the conv's raw output (after the pointwise joins), x: the saved input.  Accumulates dW (and db),
-        returns (dx or None, x_planes)."""
-        N, T, Ho, Wo, _ = gz.shape
+        returns the pair (dx or None, None)."""
         assert self.cout % 8 == 0 and gz.shape[-1] == self.cout
-        if WGRAD_PLANES:      # the first implementation: channel-major plane copies of both operands (kept for A/B runs)
-            sp = (self.pad[1], self.pad[2])
-            if x_planes is None:
-                x_planes = to.to_planes(x, pad=sp, stride=self.stride[1:], channels=self.cin, copies=True)
-            to.wgrad(to.to_planes(gz, pad=sp), x_planes, (Ho, Wo), self.k, self.g)
-        else:                 # operands read straight from NDHWC (MN-major wgmma operands, tap = TMA coordinate shift)
-            to.wgrad_nhwc(gz, x, self.k, self.stride[1:], self.g, cout=self.cout, cin=self.cin)
+        to.wgrad_nhwc(gz, x, self.k, self.stride[1:], self.g, cout=self.cout, cin=self.cin)
         if self.bias is not None:
             L.call('dt_bias_grad', L.ptr(gz), gz.numel() // gz.shape[-1], self.cout, gz.shape[-1], L.ptr(self.bias_g), L.stream_ptr())
         dx = None
@@ -140,13 +128,7 @@ class TrainConv(object):
             dx = cv.conv3d(gz, self.w_dg, self.k, (1, 1, 1), self.pad, out_f32=False, dtype=cv.BF16, cin=self.cout)
             if self.stride[1] == 2:
                 dx = to.scatter_stride2(dx, (x.shape[2], x.shape[3]))
-        return dx, x_planes
-
-    def update(self, lr, momentum, wd, grad_scale):
-        to.sgd_update(self.w, self.g, self.m, lr, momentum, wd, grad_scale, self.w_fwd, self.w_dg)
-        if self.bias is not None:     # biases: no weight decay, 2x learning rate (model_builder.py:971-976)
-            to.sgd_update(self.bias.view(1, 1, -1), self.bias_g.view(1, 1, -1), self.bias_m.view(1, 1, -1), 2.0 * lr, momentum, 0.0,
-                          grad_scale)
+        return dx, None
 
 
 class RpnTrainer(object):
@@ -373,9 +355,9 @@ class RpnTrainer(object):
             ga, _ = blk['b'].backward(gz2, sb['a'])
             gz1 = to.bwd_pointwise(ga, None, sb['a'], blk['a'].scale)
             need_dx = not last_of_trunk                                          # res2 is frozen: stop at the input of res3_0
-            gx1, xpl = blk['a'].backward(gz1, sb['x'], need_dx=need_dx)
+            gx1, _ = blk['a'].backward(gz1, sb['x'], need_dx=need_dx)
             if blk['sc'] is not None:
-                gx2, _ = blk['sc'].backward(gsc, sb['x'], x_planes=xpl, need_dx=need_dx)
+                gx2, _ = blk['sc'].backward(gsc, sb['x'], need_dx=need_dx)
             else:
                 gx2 = gsc
             for cnv in (blk['c'], blk['b'], blk['a'], blk['sc']):
@@ -430,32 +412,19 @@ class RpnTrainer(object):
 
     def _sgd_table(self):
         """One dt_sgd_item per parameter tensor (filters, then the biases: 2x learning rate, no weight decay,
-        model_builder.py:971-976) + the block prefix of the single-launch update; the pointers are stable for the trainer's life."""
-        import ctypes as C
-        torch = self.torch
-        items, first, nb = [], [], 0
-
-        def add(w, g, m, wf, wdg, taps, co, ci, lr_mult, wd_mult):
-            nonlocal nb
-            tci, tco = (ci + 31) // 32, (co + 31) // 32
-            items.append(L.SgdItem(w.data_ptr(), g.data_ptr(), m.data_ptr(), wf.data_ptr() if wf is not None else None,
-                                   wdg.data_ptr() if wdg is not None else None, taps, co, ci, tci, tco, lr_mult, wd_mult))
-            first.append(nb)
-            nb += taps * tci * tco
+        model_builder.py:971-976) for the single-launch update; the pointers are stable for the trainer's life."""
+        items = []
         for c in self.convs:
-            add(c.w, c.g, c.m, c.w_fwd, c.w_dg, c.taps, c.cout, c.cin, 1.0, 1.0)
+            items.append((c.w, c.g, c.m, c.w_fwd, c.w_dg, c.taps, c.cout, c.cin, 1.0, 1.0))
             if c.bias is not None:
-                add(c.bias, c.bias_g, c.bias_m, None, None, 1, 1, c.bias.numel(), 2.0, 0.0)
-        arr = (L.SgdItem * len(items))(*items)
-        buf = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).cuda()
-        return buf, torch.tensor(first, dtype=torch.int32).cuda(), len(items), nb
+                items.append((c.bias, c.bias_g, c.bias_m, None, None, 1, 1, c.bias.numel(), 2.0, 0.0))
+        return to.sgd_table(items)
 
     def update(self):
         gs = 1.0            # losses already carry 1/NUM_GPUS; the all-reduce is a SUM (model_builder.py:484,938-942)
         if not hasattr(self, '_sgd'):
             self._sgd = self._sgd_table()
-        buf, first, n, nb = self._sgd
-        L.call('dt_sgd_update_multi', L.ptr(buf), L.ptr(first), n, nb, float(self.lr), float(self.momentum), float(self.wd), gs, L.stream_ptr())
+        to.sgd_update_multi(self._sgd, self.lr, self.momentum, self.wd, gs)
 
     def step(self, frames_u8, targets):
         outs = self.forward_all(frames_u8)

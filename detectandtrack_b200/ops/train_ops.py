@@ -1,46 +1,9 @@
-"""Device-tensor API over csrc/train_ops.cu (training step kernels: filter gradient on the tensor cores over
-channel-major planes, elementwise backward joins, SGD update).  See include/dt_b200.h."""
+"""Device-tensor API over csrc/train_ops.cu (training step kernels: filter gradient on the tensor cores straight from
+the NDHWC tensors, elementwise backward joins, SGD update).  See include/dt_b200.h."""
 import ctypes as C
 
 from .. import _lib as L
 from . import conv as cv
-
-
-def planes_ld(Ho, Wo, pH, pW):
-    return int(L.lib().dt_planes_ld(int(Ho), int(Wo), int(pH), int(pW)))
-
-
-def to_planes(x, pad=(0, 0), stride=(1, 1), channels=None, copies=False):
-    """x [N, T, H, W, ld] bf16 -> planes [N, T, C, Pld] (zero border pad, spatial subsampling stride).
-    copies=True: the wgrad INPUT operand [2*pad_w + 1, N, T, C, Pld], copy kw pre-shifted by kw - pad_w columns."""
-    torch = L.require_cuda()
-    N, T, H, W, ld = x.shape
-    Cc = channels or ld
-    assert x.dtype == torch.bfloat16 and x.is_contiguous()
-    Ho, Wo = (H + stride[0] - 1) // stride[0], (W + stride[1] - 1) // stride[1]
-    Pld = planes_ld(Ho, Wo, pad[0], pad[1])
-    shifts = list(range(-pad[1], pad[1] + 1)) if copies else [0]
-    out = torch.empty((len(shifts), N, T, Cc, Pld), dtype=torch.bfloat16, device='cuda')
-    L.call('dt_to_planes', L.ptr(x), N * T, H, W, Cc, ld, stride[0], stride[1], pad[0], pad[1], shifts[0], len(shifts), L.ptr(out),
-           L.stream_ptr())
-    return out if copies else out[0]
-
-
-def wgrad(gz_planes, x_planes, out_hw, ksize, dW=None):
-    """gz_planes [N,T,Cout,Pld], x_planes [kW,N,T,Cin,Pld] (to_planes(copies=True), pad = k // 2) -> dW [taps, Cout, Cin] fp32
-    (accumulated into `dW` if given, else a zeroed buffer)."""
-    torch = L.require_cuda()
-    N, T, Cout, Pld = gz_planes.shape
-    kT, kH, kW = ksize
-    assert x_planes.dim() == 5 and x_planes.shape[0] == kW, 'x_planes: to_planes(..., copies=True) -> [kW, N, T, Cin, Pld]'
-    Cin = x_planes.shape[3]
-    assert x_planes.shape[1] == N and x_planes.shape[2] == T and x_planes.shape[4] == Pld and x_planes.is_contiguous()
-    assert Pld == planes_ld(out_hw[0], out_hw[1], kH // 2, kW // 2)
-    if dW is None:
-        dW = L.zeros((kT * kH * kW, Cout, Cin), torch.float32)
-    assert dW.dtype == torch.float32 and tuple(dW.shape) == (kT * kH * kW, Cout, Cin) and dW.is_contiguous()
-    L.call('dt_wgrad', L.ptr(gz_planes), L.ptr(x_planes), N, T, out_hw[0], out_hw[1], Cout, Cin, kT, kH, kW, L.ptr(dW), L.stream_ptr())
-    return dW
 
 
 def wgrad_nhwc(gz, x, ksize, stride=(1, 1), dW=None, cout=None, cin=None):
@@ -95,11 +58,35 @@ def scatter_stride2(src, hw):
     return out
 
 
+def sgd_table(items):
+    """The dt_sgd_item table of dt_sgd_update_multi, on the device: items are (w, g, m, w_fwd, w_dgrad, taps, Cout, Cin,
+    lr_mult, wd_mult) with w / g / m fp32 [taps, Cout, Cin] and the bf16 forward / dgrad filters (or None) to refresh
+    -> (items buffer, first_block, n_items, total_blocks).  The table holds raw pointers: the tensors must outlive it."""
+    torch = L.require_cuda()
+    rows, first, nb = [], [], 0
+    for w, g, m, wf, wdg, taps, co, ci, lr_mult, wd_mult in items:
+        tci, tco = (ci + 31) // 32, (co + 31) // 32
+        rows.append(L.SgdItem(w.data_ptr(), g.data_ptr(), m.data_ptr(), wf.data_ptr() if wf is not None else None,
+                              wdg.data_ptr() if wdg is not None else None, taps, co, ci, tci, tco, lr_mult, wd_mult))
+        first.append(nb)
+        nb += taps * tci * tco
+    arr = (L.SgdItem * len(rows))(*rows)
+    buf = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).cuda()
+    return buf, torch.tensor(first, dtype=torch.int32).cuda(), len(rows), nb
+
+
+def sgd_update_multi(table, lr, momentum, wd, grad_scale=1.0):
+    """MomentumSGDUpdate of every item of an sgd_table in one launch; refreshes the bf16 forward / dgrad filters."""
+    buf, first, n, nb = table
+    L.call('dt_sgd_update_multi', L.ptr(buf), L.ptr(first), n, nb, float(lr), float(momentum), float(wd), float(grad_scale),
+           L.stream_ptr())
+
+
 def sgd_update(w, g, m, lr, momentum=0.9, wd=1e-4, grad_scale=1.0, w_fwd=None, w_dgrad=None):
-    """MomentumSGDUpdate on packed fp32 master weights [taps, Cout, Cin]; refreshes the bf16 forward / dgrad filters."""
+    """MomentumSGDUpdate of one packed fp32 master filter [taps, Cout, Cin] (dt_sgd_update_multi over a one-item table);
+    refreshes the bf16 forward / dgrad filters if given."""
     taps, Cout, Cin = w.shape
-    L.call('dt_sgd_update', L.ptr(w), L.ptr(g), L.ptr(m), taps, Cout, Cin, float(lr), float(momentum), float(wd), float(grad_scale),
-           L.ptr(w_fwd), L.ptr(w_dgrad), L.stream_ptr())
+    sgd_update_multi(sgd_table([(w, g, m, w_fwd, w_dgrad, taps, Cout, Cin, 1.0, 1.0)]), lr, momentum, wd, grad_scale)
 
 
 def pack_dgrad_weight(w):

@@ -436,33 +436,17 @@ int dt_fold_tube_heads(const float* in, int ld, int R, int T, int C, float* cls,
  * NCCL / muji all-reduce of the per-GPU gradients (lib/modeling/model_builder.py:908-985).  Here:
  *   dgrad   of a stride-1 'same' conv = dt_conv3d of the gradient with the flipped, transposed filter (w_dgrad below);
  *           stride-2 pointwise convs: dt_conv3d on the coarse map + dt_scatter_stride2
- *   wgrad   dt_wgrad on channel-major planes (dt_to_planes) of the gradient and of the saved input
+ *   wgrad   dt_wgrad_nhwc, both operands read straight from the NDHWC gradient and saved input
  *   the elementwise joins (Relu / Sum / AffineChannelNd gradient, lib/ops/affine_channel_nd_op.cu:73-92) dt_bwd_pointwise,
- *   the FPN top-down join dt_upsample_add_bwd, the update dt_sgd_update.  All tensors bf16 unless noted. */
+ *   the FPN top-down join dt_upsample_add_bwd, the update dt_sgd_update_multi (every parameter tensor in one launch).
+ *   All tensors bf16 unless noted. */
 
-/* positions of one channel-major plane of an Ho x Wo map with a zero border pH / pW: (Ho + 2 pH) rows of Wp = (Wo + 2 pW)
- * rounded up to 8 positions (so a filter-row offset keeps TMA's 16-byte coordinate alignment) */
-int dt_planes_ld(int Ho, int Wo, int pH, int pW);
-
-/* x [F = N*T frames, H, W, ldx] (first C channels) -> planes [F, C, dt_planes_ld(Ho, Wo, pH, pW)], Ho = ceil(H / sh),
- * Wo = ceil(W / sw): plane position (ho + pH) * Wp + wo + pW - wshift holds x[f, ho*sh, wo*sw, c]; border and tail zero.
- * wshift in [-pW, pW]: the copy in which column c holds the pixel of column c + wshift (dt_wgrad's operand for kw = pW + wshift).
- * ncopies >= 1 consecutive shifts wshift .. wshift + ncopies - 1 are written to out [ncopies][F, C, Pld] from one staged read. */
-int dt_to_planes(const void* x, int F, int H, int W, int C, int ldx, int sh, int sw, int pH, int pW, int wshift, int ncopies,
-                 void* out, void* stream);
-
-/* Filter gradient of a stride-1 'same' conv (odd kT/kH/kW, pads k/2): dW [kT*kH*kW][Cout][Cin] fp32 +=
- * sum_{n,t,h,w} gz[n,t,h,w,co] * x[n, t+kt-pT, h+kh-pH, w+kw-pW, ci].  gz_planes [N*T, Cout, Pld] (wshift 0), x_planes
- * [kW][N*T, Cin, Pld]: copy kw from dt_to_planes with pH = kH/2, pW = kW/2, wshift = kw - pW (strided 1x1 convs: x
- * subsampled by dt_to_planes).
- * dW (8-byte aligned) is ACCUMULATED into (split-K partial sums, red.global): the caller zeroes it (dt_memset). */
-int dt_wgrad(const void* gz_planes, const void* x_planes, int N, int T, int Ho, int Wo, int Cout, int Cin, int kT, int kH, int kW,
-             float* dW, void* stream);
-
-/* The same filter gradient read straight from the NDHWC tensors (no planes): gz [N, T, Ho, Wo, ld_g] (first Cout channels),
- * x [N, T, Hi, Wi, ld_x] (first Cin channels), both bf16.  Positions are the K axis of MN-major wgmma operands staged by
- * 5-D TMA boxes; the tap is a coordinate shift (zero fill = padding).  sH / sW > 1 only for pointwise convs
- * (Ho = ceil(Hi / sH)).  dW [taps][Cout][Cin] fp32, 8-byte aligned, is accumulated into (caller zeroes). */
+/* Filter gradient of a 'same' conv (odd kT/kH/kW, pads k/2): dW [kT*kH*kW][Cout][Cin] fp32 +=
+ * sum_{n,t,h,w} gz[n,t,h,w,co] * x[n, t+kt-pT, h+kh-pH, w+kw-pW, ci], read straight from the NDHWC tensors:
+ * gz [N, T, Ho, Wo, ld_g] (first Cout channels), x [N, T, Hi, Wi, ld_x] (first Cin channels), both bf16.  Positions are
+ * the K axis of MN-major wgmma operands staged by 5-D TMA boxes; the tap is a coordinate shift (zero fill = padding).
+ * sH / sW > 1 only for pointwise convs (Ho = ceil(Hi / sH)).  dW (8-byte aligned) is ACCUMULATED into (split-K partial
+ * sums, red.global): the caller zeroes it (dt_memset). */
 int dt_wgrad_nhwc(const void* gz, int ld_g, const void* x, int ld_x, int N, int T, int Ho, int Wo, int Hi, int Wi, int Cout, int Cin,
                   int kT, int kH, int kW, int sH, int sW, float* dW, void* stream);
 
@@ -492,15 +476,13 @@ int dt_upsample_add_bwd(const void* fine, const void* coarse_in, int F, int Hc, 
 /* out [F, H, W, C] = zeros except out[f, 2h, 2w] = src[f, h, w]; src [F, ceil(H/2), ceil(W/2), C] */
 int dt_scatter_stride2(const void* src, int F, int Hs, int Ws, int H, int W, int C, void* out, void* stream);
 
-/* Caffe2 MomentumSGDUpdate + weight decay (model_builder.py:954-985): g' = lr * (grad_scale * g + wd * w) + momentum * m;
- * m = g'; w -= g'.  w / g / m fp32 [taps][Cout][Cin] (the packed order of dt_conv3d's filter).  w_fwd_bf16 (may be NULL)
- * receives the new filter as bf16 in the same order, w_dgrad_bf16 (may be NULL) the dgrad filter [taps (flipped)][Cin][Cout]. */
-int dt_sgd_update(float* w, const float* g, float* m, int taps, int Cout, int Cin, float lr, float momentum, float wd,
-                  float grad_scale, void* w_fwd_bf16, void* w_dgrad_bf16, void* stream);
-
-/* The same update for EVERY parameter tensor in one launch.  items: device array of dt_sgd_item; first_block [n_items]: device,
- * exclusive prefix of taps * ceil(Cout/32) * ceil(Cin/32) per item; total_blocks = their sum.  Per item the learning rate is
- * lr * lr_mult and the weight decay wd * wd_mult (biases: 2x / 0, model_builder.py:971-976). */
+/* Caffe2 MomentumSGDUpdate + weight decay (model_builder.py:954-985) of EVERY parameter tensor in one launch:
+ * g' = lr * (grad_scale * g + wd * w) + momentum * m;  m = g';  w -= g'.  Per item w / g / m are fp32 [taps][Cout][Cin]
+ * (the packed order of dt_conv3d's filter); w_fwd_bf16 (may be NULL) receives the new filter as bf16 in the same order,
+ * w_dgrad_bf16 (may be NULL) the dgrad filter [taps (flipped)][Cin][Cout].  items: device array of dt_sgd_item;
+ * first_block [n_items]: device, exclusive prefix of taps * ceil(Cout/32) * ceil(Cin/32) per item; total_blocks = their
+ * sum.  Per item the learning rate is lr * lr_mult and the weight decay wd * wd_mult (biases: 2x / 0,
+ * model_builder.py:971-976). */
 typedef struct dt_sgd_item {
   float* w; const float* g; float* m; void* w_fwd_bf16; void* w_dgrad_bf16;
   int taps, Cout, Cin, tiles_ci, tiles_co;

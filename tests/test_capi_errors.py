@@ -49,14 +49,14 @@ def _cases():
         ('dt_frame_costs', (None, 3, 1, None, 0, 0, 0, 0, 0.5, None, None, 2, 4, 1.0, 0.0, None, None), b'dt_frame_costs'),
         ('dt_pairs_to_f16', (None, 10, 12, None, None), b'C % 8'),
         ('dt_scale_rois', (None, 2, 10, 4, None, 1, 1.0, None, None), b'dt_scale_rois'),
-        ('dt_to_planes', (None, 1, 8, 8, 12, 12, 1, 1, 0, 0, 0, 1, None, None), b'dt_to_planes'),
-        ('dt_wgrad', (None, None, 1, 1, 8, 8, 64, 60, 1, 3, 3, None, None), b'Cin % 8'),
+        ('dt_wgrad_nhwc', (None, 64, None, 64, 1, 1, 8, 8, 8, 8, 64, 64, 1, 3, 3, 2, 2, None, None), b'only pointwise'),
+        ('dt_wgrad_nhwc', (None, 64, None, 64, 1, 1, 4, 4, 8, 8, 64, 64, 1, 1, 1, 1, 1, None, None), b'does not match'),
         ('dt_wgrad_nhwc', (None, 64, None, 60, 1, 1, 8, 8, 8, 8, 64, 60, 1, 3, 3, 1, 1, None, None), b'dt_wgrad_nhwc'),
         ('dt_bwd_pointwise', (None, None, None, None, 10, 12, None, None), b'C % 8'),
         ('dt_bwd_pointwise2', (None, None, None, None, 10, 12, None, None, None, None), b'C % 8'),
         ('dt_upsample_add_bwd', (None, None, 1, 4, 4, 12, None, None), b'dt_upsample_add_bwd'),
         ('dt_scatter_stride2', (None, 1, 4, 4, 9, 8, 64, None, None), b'dt_scatter_stride2'),
-        ('dt_sgd_update', (None, None, None, 1, 8, 8, 0.1, 0.9, 0.0, 1.0, None, None, None), b'dt_sgd_update'),
+        ('dt_sgd_update_multi', (None, None, 1, 1, 0.1, 0.9, 0.0, 1.0, None), b'null pointer'),
         ('dt_sgd_update_multi', (None, None, 0, 0, 0.1, 0.9, 0.0, 1.0, None), b'empty table'),
         ('dt_bias_grad', (None, 10, 12, 16, None, None), b'dt_bias_grad'),
         ('dt_rpn_loss_grad', (None, 8, None, None, None, None, 10, 3, 1.0, 1.0, 0.1, None, 16, None, None), b'dt_rpn_loss_grad'),

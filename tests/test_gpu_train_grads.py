@@ -37,8 +37,8 @@ def _ints(torch, g, shape, a):
 
 
 def _conv(torch, r, seed, wa=3):
-    """A TrainConv of the row's shape with integer weights (the bf16 forward / dgrad filters re-emitted by dt_sgd_update at
-    lr 0, as the trainer refreshes them), its gradient a view at an 8-byte (not 16-byte) offset of a flat buffer like the
+    """A TrainConv of the row's shape with integer weights (the bf16 forward / dgrad filters re-emitted by dt_sgd_update_multi
+    at lr 0, as the trainer refreshes them), its gradient a view at an 8-byte (not 16-byte) offset of a flat buffer like the
     trainer's, pre-filled with integers."""
     from detectandtrack_b200.modeling.trainer import TrainConv
     from detectandtrack_b200.ops import train_ops as to

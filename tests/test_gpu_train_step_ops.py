@@ -513,21 +513,6 @@ def _sgd_items(tr, n):
     return items[:n]
 
 
-def _launch_sgd_table(L, shapes, bufs, lr, mu, wd, gs):
-    """An SgdItem table over the given per-item buffers, launched once."""
-    it, first, nb = [], [], 0
-    for (taps, co, ci, lm, wm), (w, g, m, wf, wdg) in zip(shapes, bufs):
-        tci, tco = (ci + 31) // 32, (co + 31) // 32
-        it.append(L.SgdItem(w.data_ptr(), g.data_ptr(), m.data_ptr(), wf.data_ptr() if wf is not None else None,
-                             wdg.data_ptr() if wdg is not None else None, taps, co, ci, tci, tco, lm, wm))
-        first.append(nb)
-        nb += taps * tci * tco
-    arr = (L.SgdItem * len(it))(*it)
-    buf = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).cuda()
-    fb = torch.tensor(first, dtype=torch.int32).cuda()
-    L.call('dt_sgd_update_multi', L.ptr(buf), L.ptr(fb), len(it), nb, lr, mu, wd, gs, L.stream_ptr())
-
-
 def _check_sgd_item(w0, g0, m0, w, m, wf, wdg, lr, mu, wd, gs, lm, wm, what):
     nw, nm, bw, bm = sgd_ref(w0, g0, m0, lr, mu, wd, gs, lm, wm)
     r = max(_within(w, nw, bw, what + ' w'), _within(m, nm, bm, what + ' m'))
@@ -544,7 +529,7 @@ def test_sgd_update_multi_step_table(step_env, key, record_property):
     filters of Cout / Cin 16, 72 and the 1-row biases included, with nonzero momentum, each copy in one flat buffer per
     operand behind a sentinel gap: w and m within sgd_ref's bound, the bf16 forward and dgrad filters equal to bf16(w) and
     its flipped transpose, and every sentinel intact (no item moved twice, nothing outside an item written)."""
-    from detectandtrack_b200 import _lib as L
+    from detectandtrack_b200.ops import train_ops as to
     tr = step_env['tr']
     items = _sgd_items(tr, key[0])
     assert len(items) == key[0]
@@ -564,7 +549,7 @@ def test_sgd_update_multi_step_table(step_env, key, record_property):
         off += n + gap
     snap = {k: flat[k].clone() for k in flat}
     bufs = [(v['w'], v['g'], v['m'], v['f'] if hw else None, v['d'] if hw else None) for v, hw, _, _ in views]
-    _launch_sgd_table(L, shapes, bufs, f32(tr.lr), f32(tr.momentum), f32(tr.wd), 1.0)
+    to.sgd_update_multi(to.sgd_table([b + s for b, s in zip(bufs, shapes)]), f32(tr.lr), f32(tr.momentum), f32(tr.wd), 1.0)
     torch.cuda.synchronize()
     worst = 0.0
     mask = torch.ones(total, dtype=torch.bool, device='cuda')

@@ -4,7 +4,6 @@ dt_wgrad_nhwc_plan / dt_conv_plan.  The reduced shapes below are what tests/test
 that each one takes the step's plan.  Also: the fp64 tap-sum references of that file against torch autograd, and the host
 alignment checks of the backward entry points."""
 import ctypes as C
-import os
 
 import pytest
 
@@ -277,10 +276,6 @@ def dgrad_ref(gz, w, k, in_hw, s=(1, 1)):
 
 
 # ---------------------------------------------------------------------------------------------------- tests
-def test_no_wave_override():
-    assert 'DT_WGRAD_WAVES' not in os.environ, 'DT_WGRAD_WAVES changes the K split of every wgrad plan'
-
-
 def test_table_lists_exactly_the_launches_the_step_makes():
     assert len(ROWS) == len(TRAIN_STEP)
     no_dgrad = {r[0] for r in TRAIN_STEP if 'd' not in r[9]}
@@ -373,7 +368,6 @@ def _p(a):
 
 ALIGN_CASES = [
     ('dt_wgrad_nhwc', (_p(0x1000), 64, _p(0x1000), 64, 1, 1, 8, 8, 8, 8, 64, 64, 1, 1, 1, 1, 1, _p(0x1004), None), b'8-byte'),
-    ('dt_wgrad', (_p(0x1000), _p(0x1000), 1, 1, 8, 8, 64, 64, 1, 1, 1, _p(0x1004), None), b'8-byte'),
     ('dt_bias_grad', (_p(0x1008), 10, 16, 16, _p(0x1000), None), b'16-byte'),
     ('dt_bwd_pointwise', (_p(0x1000), _p(0x1008), None, None, 10, 16, _p(0x1000), None), b'16-byte'),
     ('dt_bwd_pointwise2', (_p(0x1000), None, _p(0x1000), None, 10, 16, _p(0x1000), None, _p(0x1002), None), b'16-byte'),

@@ -1,7 +1,7 @@
-"""Micro-benchmark of the wgmma filter-gradient kernels on the trainable layer shapes of the keypoint R-CNN training step at
-TRAIN.IMS_PER_BATCH = 2 clips (T = 3, 800x1344 blob): dt_wgrad_nhwc (operands straight from NDHWC, the path the trainer uses)
-next to the first implementation (dt_to_planes + dt_wgrad).  CUDA events, median of --iters; TFLOP/s = 2*MACs of the conv.
-    python tools/bench_wgrad.py [--iters 5] [--only res4] [--planes]"""
+"""Micro-benchmark of the wgmma filter-gradient kernel dt_wgrad_nhwc on the trainable layer shapes of the keypoint R-CNN
+training step at TRAIN.IMS_PER_BATCH = 2 clips (T = 3, 800x1344 blob).  CUDA events, median of --iters; TFLOP/s = 2*MACs
+of the conv.
+    python tools/bench_wgrad.py [--iters 5] [--only res4]"""
 import argparse
 import json
 import os
@@ -33,7 +33,6 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--iters', type=int, default=5)
     ap.add_argument('--only', default='')
-    ap.add_argument('--planes', action='store_true', help='also time the plane-copy implementation')
     a = ap.parse_args()
     rows = []
     for name, N, T, H, W, Cin, Cout, k in LAYERS:
@@ -53,22 +52,6 @@ def main():
             ts.append(e0.elapsed_time(e1))
         ms = sorted(ts)[len(ts) // 2]
         row = dict(layer=name, wgrad_nhwc_ms=round(ms, 4), tflops=round(fl / ms / 1e9, 1), gflop=round(fl / 1e9, 1))
-        if a.planes:
-            pad = (k[1] // 2, k[2] // 2)
-            xp = to.to_planes(x, pad=pad, copies=True)
-            gp = to.to_planes(gz, pad=pad)
-            dW2 = to.wgrad(gp, xp, (H, W), k)
-            torch.cuda.synchronize()
-            ts, tp = [], []
-            for _ in range(a.iters):
-                e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
-                e0.record()
-                xp = to.to_planes(x, pad=pad, copies=True); gp = to.to_planes(gz, pad=pad)
-                e1.record()
-                to.wgrad(gp, xp, (H, W), k, dW2)
-                e2.record(); torch.cuda.synchronize()
-                tp.append(e0.elapsed_time(e1)); ts.append(e1.elapsed_time(e2))
-            row.update(planes_wgrad_ms=round(sorted(ts)[len(ts) // 2], 4), planes_copy_ms=round(sorted(tp)[len(tp) // 2], 4))
         rows.append(row)
         print(json.dumps(rows[-1]), flush=True)
     os.makedirs('gpurun_out', exist_ok=True)
