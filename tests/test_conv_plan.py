@@ -134,11 +134,6 @@ def plan_key(dtype, x3, out_f32, res_mode, o):
     return (dtype, x3, out_f32, res_mode) + tuple(getattr(o, f) for f in PLAN_FIELDS)
 
 
-def table_plan_keys():
-    return {plan_key(a['dtype'], a['x3'], a['out_f32'], l[10], step_plan(l, m))
-            for l in R50_FPN_3D for m in layer_modes(l) for a in [conv_args(l, m)]}
-
-
 @pytest.mark.parametrize('layer', R50_FPN_3D, ids=[l[0] for l in R50_FPN_3D])
 def test_plan_of_every_bench_layer_fits_and_fills_the_mma(layer):
     name, N, T, H, W, Cin, Cout, k, s, p, rm = layer

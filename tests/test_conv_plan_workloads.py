@@ -1,7 +1,7 @@
 """CPU: the conv launches of the other benchmarked workloads, through dt_conv_plan (no GPU needed).  test_conv_plan.py
 pins the R50-FPN-3D inference step; this file adds the 2-D R50-FPN inference step (`bench.py --config r50fpn2d`), the
 R18-3D tube step (`--config r18tube`) and the forward convs of the keypoint R-CNN training step, each at the reduced
-shapes tests/test_gpu_conv_workloads.py runs, and the stricter launch key that the coverage spy of that file checks."""
+shapes tests/test_gpu_conv_workloads.py runs, and the stricter launch key that the coverage test of that file checks."""
 import pytest
 
 from test_conv_plan import PLAN_FIELDS, R50_FPN_3D, SMS, conv_args, layer_modes, plan_key, step_plan

@@ -1,6 +1,6 @@
 """GPU: every launch key of the box stages on the benchmarked steps (dt_rpn_proposals_multi, dt_nms_batched, dt_collect_rpn,
 dt_distribute_fpn, dt_box_decode, dt_limit_detections, dt_rpn_targets, dt_sample_rois), launched at the step's shapes and
-compared exactly with the host references of tests/test_box_reference.py and oracle/, plus a spy test that proves the table
+compared exactly with the host references of tests/test_box_reference.py and oracle/, plus a coverage test that proves the table
 lists every key DetectionEngine.detect (r50fpn3d, r50fpn2d, r18tube, every dtype the engine takes) and KeypointRcnnTrainer.step
 launch, and a teacher-forced capture of the real steps whose downstream stages are re-run by the oracle on the device's own
 upstream output.
@@ -82,61 +82,27 @@ def _train_cfg():
     return cfg
 
 
-def test_step_box_ops_are_all_in_the_table(monkeypatch, record_property):
+def test_step_box_ops_are_all_in_the_table(record_property):
     """One 800 x 1333 clip of each bench workload through DetectionEngine.detect in bf16, bf16x3, bf16x3h and tf32x3 (where
     the engine takes them), and one KeypointRcnnTrainer.step at the bench training config: every launch of the box entry
     points has a key in TABLE, each of which has a value test below."""
-    import bench
-    from detectandtrack_b200 import _lib as L
-    from detectandtrack_b200.modeling import params as Pm
-    from detectandtrack_b200.modeling.engine import DetectionEngine
-    from detectandtrack_b200.modeling.trainer import KeypointRcnnTrainer, pack_gt
-    launched = []
-    orig_call = L.call
-
-    def spy(name, *a):
-        k = launch_key(name, a)
-        if k is not None:
-            launched.append((name, k))
-        return orig_call(name, *a)
-    monkeypatch.setattr(L, 'call', spy)
+    import step_launches as sl
     missing, seen = {}, set()
-    try:
-        for wl in ('r50fpn3d', 'r50fpn2d', 'r18tube'):
-            cfg = bench.bench_cfg(800, 1333, wl)
-            blobs, spec = Pm.random_blobs(cfg)
-            frames = torch.from_numpy(bench.synth_frames(1, bench.frames_per_clip(cfg), 800, 1333, 7)).cuda()
-            for mode in ('bf16', 'bf16x3', 'bf16x3h', 'tf32x3'):
-                del launched[:]
-                try:
-                    eng = DetectionEngine(cfg, blobs, spec, dtype=mode)
-                except NotImplementedError:
-                    assert mode not in ('bf16', 'bf16x3'), (wl, mode)
-                    continue
-                eng.detect(frames)
-                torch.cuda.synchronize()
-                names = {n for n, _ in launched}
-                assert {'dt_rpn_proposals_multi', 'dt_nms_batched', 'dt_collect_rpn', 'dt_box_decode', 'dt_limit_detections'} <= names
-                for name, k in launched:
-                    seen.add((name, k))
-                    if k not in TABLE[name]:
-                        missing.setdefault((name, k), (wl, mode))
-                del eng
-        cfg = _train_cfg()
-        blobs, spec = Pm.random_blobs(cfg)
-        tr = KeypointRcnnTrainer(cfg, blobs, spec)
-        frames = torch.from_numpy(bench.synth_frames(2, 3, 800, 1333, 5)).cuda()
-        del launched[:]
-        tr.step(frames, pack_gt(bench.synth_gt(2, 800, 1333, 11)), seed=9)
-        torch.cuda.synchronize()
-        assert {'dt_rpn_targets', 'dt_sample_rois'} <= {n for n, _ in launched}
+    for run in [(wl, m) for wl in sl.WORKLOADS for m in ('bf16', 'bf16x3', 'bf16x3h', 'tf32x3')] + ['train']:
+        rec = sl.record(run)
+        if not rec.taken:
+            assert run[1] not in ('bf16', 'bf16x3'), run
+            continue
+        launched = [(name, k) for name, a, _ in rec.calls if (k := launch_key(name, a)) is not None]
+        names = {n for n, _ in launched}
+        if run == 'train':
+            assert {'dt_rpn_targets', 'dt_sample_rois'} <= names
+        else:
+            assert {'dt_rpn_proposals_multi', 'dt_nms_batched', 'dt_collect_rpn', 'dt_box_decode', 'dt_limit_detections'} <= names
         for name, k in launched:
             seen.add((name, k))
             if k not in TABLE[name]:
-                missing.setdefault((name, k), ('train', 'bf16'))
-    finally:
-        from test_gpu_engine import _cfg
-        _cfg()
+                missing.setdefault((name, k), run)
     record_property('keys_seen', len(seen))
     print('box keys seen: %d' % len(seen))
     for s in sorted(seen, key=str):

@@ -699,63 +699,3 @@ def test_exact_check_names_a_wrong_lo_box(mode, monkeypatch):
     msg = _exact_mismatch(y, ref_in, layer[8], layer[9], 'wrong lo box')
     assert msg is not None and 'x_lo*w_hi of tap (0, 0, 0), k-block 1 dropped' in msg, msg
 
-
-def test_step_convs_are_all_in_the_table(monkeypatch, record_property):
-    """One 800 x 1333 clip of the benchmarked R50-FPN-3D config through DetectionEngine.detect in bf16, bf16x3,
-    bf16x3h and tf32x3: every conv_tc launch has a plan key (storage, residual kind, BN, schedule length, ring, staging
-    and residual split) of a test_conv_plan.R50_FPN_3D layer, which the value test above checks at three or more tiles
-    per CTA; every conv1 launch runs a variant test_conv1_packed_rows_vs_torch / test_conv1_exact_fp32_vs_fp64 check."""
-    import ctypes as C
-    import torch
-    import bench
-    from detectandtrack_b200 import _lib as L
-    from detectandtrack_b200.modeling import params as P
-    from detectandtrack_b200.modeling.engine import DetectionEngine
-    from detectandtrack_b200.ops import conv as cv
-    from test_conv_plan import plan_key, table_plan_keys
-    table = table_plan_keys()
-    conv1_tested = {('conv1', 0, 1, 0), ('conv1', 0, 0, 0), ('conv1', 1, 1, 0), ('conv1', 0, 0, 1), ('conv1_f32', 0)}
-    calls, launched = {'py': 0, 'c': 0}, []
-    orig_call = L.call
-
-    def spy(name, *a):
-        if name == 'dt_conv3d':
-            d = a[0]._obj
-            o = L.ConvPlan()
-            aligned = a[5] is None or a[5].value % 16 == 0
-            assert L.lib().dt_conv_plan(C.byref(d), int(aligned), C.byref(o)) == 0, L.lib().dt_last_error()
-            launched.append((plan_key(d.dtype, d.x3, d.out_f32, d.res_mode, o), (d.N, d.Ti, d.Hi, d.Wi, d.Cin, d.Cout)))
-        elif name == 'dt_conv1_7x7s2':
-            launched.append((('conv1', a[10], a[11], a[13]), None))
-        elif name == 'dt_conv1_7x7s2_f32':
-            launched.append((('conv1_f32', a[8]), None))
-        if name.startswith(('dt_conv3d', 'dt_conv1_7x7s2')):
-            calls['c'] += 1
-        return orig_call(name, *a)
-
-    def counted(f):
-        def wrapped(*a, **kw):
-            calls['py'] += 1
-            return f(*a, **kw)
-        return wrapped
-    monkeypatch.setattr(L, 'call', spy)
-    for f in ('conv3d', 'conv1_7x7s2', 'conv1_7x7s2_f32'):
-        monkeypatch.setattr(cv, f, counted(getattr(cv, f)))
-    cfg = bench.bench_cfg(800, 1333)
-    blobs, spec = P.random_blobs(cfg)
-    frames = torch.from_numpy(bench.synth_frames(1, bench.frames_per_clip(cfg), 800, 1333, 7)).cuda()
-    missing = {}
-    for mode in ('bf16', 'bf16x3', 'bf16x3h', 'tf32x3'):
-        del launched[:]
-        eng = DetectionEngine(cfg, blobs, spec, dtype=mode)
-        eng.detect(frames)
-        torch.cuda.synchronize()
-        assert len(launched) > 50
-        record_property('launches_' + mode, len(launched))
-        record_property('plan_keys_' + mode, len({k for k, _ in launched}))
-        for key, shape in launched:
-            if key not in table and key not in conv1_tested:
-                missing.setdefault(key, (mode, shape))
-        del eng
-    assert calls['py'] == calls['c']
-    assert not missing, missing

@@ -1,7 +1,8 @@
 """GPU: every conv plan of the 2-D R50-FPN step (`bench.py --config r50fpn2d`), the R18-3D tube step (`--config r18tube`)
 and the forward of the keypoint R-CNN training step, at several tiles per CTA, against the fp64 tap-sum reference; and a
-spy over those steps (and R50-FPN-3D in tf32) that every launch they make is one of the value-tested plans, by the
-stricter key of test_conv_plan_workloads.plan_key_v2 (which tells strided and stacked launches apart)."""
+check over those steps and the R50-FPN-3D step (tests/step_launches.py records them) that every launch they make is one
+of the value-tested plans, by the stricter key of test_conv_plan_workloads.plan_key_v2 (which tells strided and stacked
+launches apart)."""
 import pytest
 
 from test_conv_plan import step_plan
@@ -35,103 +36,49 @@ def test_strided_conv_on_32_image_stacks_vs_fp64(mode, operands, record_property
                      operands)
 
 
-def test_workload_convs_are_all_in_the_tables(monkeypatch, record_property):
-    """One 800 x 1333 clip of r50fpn2d and of r18tube through DetectionEngine.detect in every mode bench.py times
-    (bf16x3, bf16x3h, bf16, tf32) and tf32x3, one r50fpn3d clip in tf32, and one KeypointRcnnTrainer.step at the bench
-    training config: every dt_conv3d launch (of the training step: every forward launch, outside TrainConv.backward) has
-    the plan_key_v2 of a row of test_conv_plan.R50_FPN_3D or of a test_conv_plan_workloads table, each value-tested
-    above or in test_gpu_conv.py; every conv1 launch runs a variant the conv1 tests of test_gpu_conv.py check."""
-    import ctypes as C
-    import torch
-    import bench
-    from detectandtrack_b200 import _lib as L
-    from detectandtrack_b200.modeling import params as P
-    from detectandtrack_b200.modeling.engine import DetectionEngine
-    from detectandtrack_b200.modeling.trainer import KeypointRcnnTrainer, TrainConv, pack_gt
-    from detectandtrack_b200.ops import conv as cv
+def test_workload_convs_are_all_in_the_tables(record_property):
+    """One 800 x 1333 clip of each bench workload through DetectionEngine.detect in every mode (where the engine takes
+    it), and one KeypointRcnnTrainer.step at the bench training config: every dt_conv3d launch (of the training step:
+    every forward launch, outside TrainConv.backward) has the plan_key_v2 of a row of test_conv_plan.R50_FPN_3D or of a
+    test_conv_plan_workloads table, each value-tested above or in test_gpu_conv.py; every conv1 launch runs a variant the
+    conv1 tests of test_gpu_conv.py check."""
+    import step_launches as sl
     table = {}
     for wl in ('r50fpn3d',) + tuple(TABLES):
         for k, rows in table_keys(wl).items():
             table.setdefault(k, []).extend(rows)
     conv1_tested = {('conv1', 0, 1, 0), ('conv1', 0, 0, 0), ('conv1', 1, 1, 0), ('conv1', 0, 0, 1), ('conv1_f32', 0)}
-    calls, launched, state = {'py': 0, 'c': 0}, [], dict(bwd=0)
-    orig_call = L.call
-
-    def spy(name, *a):
-        if name.startswith(('dt_conv3d', 'dt_conv1_7x7s2')):
-            calls['c'] += 1
-        if state['bwd']:
-            return orig_call(name, *a)
-        if name == 'dt_conv3d':
-            d = a[0]._obj
-            o = L.ConvPlan()
-            aligned = a[5] is None or a[5].value % 16 == 0
-            assert L.lib().dt_conv_plan(C.byref(d), int(aligned), C.byref(o)) == 0, L.lib().dt_last_error()
-            key = plan_key_v2(d.dtype, d.x3, d.out_f32, d.res_mode, o, (d.kT, d.kH, d.kW), (d.sT, d.sH, d.sW))
-            launched.append((key, (d.N, d.Ti, d.Hi, d.Wi, d.Cin, d.Cout)))
-        elif name == 'dt_conv1_7x7s2':
-            launched.append((('conv1', a[10], a[11], a[13]), None))
-        elif name == 'dt_conv1_7x7s2_f32':
-            launched.append((('conv1_f32', a[8]), None))
-        return orig_call(name, *a)
-
-    def counted(f):
-        def wrapped(*a, **kw):
-            calls['py'] += 1
-            return f(*a, **kw)
-        return wrapped
-    bw = TrainConv.backward
-
-    def backward(self, *a, **kw):
-        state['bwd'] += 1
-        try:
-            return bw(self, *a, **kw)
-        finally:
-            state['bwd'] -= 1
-    monkeypatch.setattr(L, 'call', spy)
-    monkeypatch.setattr(TrainConv, 'backward', backward)
-    for f in ('conv3d', 'conv1_7x7s2', 'conv1_7x7s2_f32'):
-        monkeypatch.setattr(cv, f, counted(getattr(cv, f)))
+    calls = {'py': 0, 'c': 0}
     missing, seen = {}, set()
-
-    def check(tag):
+    for run in sl.ENGINE_RUNS + ('train',):
+        rec = sl.record(run)
+        tag = 'train_forward' if run == 'train' else '%s_%s' % run
+        if not rec.taken:
+            assert run[1] not in ('bf16', 'bf16x3'), run
+            record_property('not_taken_' + tag, True)
+            continue
+        calls['py'] += rec.conv_py
+        launched = []
+        for name, a, in_backward in rec.calls:
+            if name.startswith(('dt_conv3d', 'dt_conv1_7x7s2')):
+                calls['c'] += 1
+            if in_backward:
+                continue
+            if name == 'dt_conv3d':
+                d, o = sl.conv_plan(a)
+                key = plan_key_v2(d.dtype, d.x3, d.out_f32, d.res_mode, o, (d.kT, d.kH, d.kW), (d.sT, d.sH, d.sW))
+                launched.append((key, (d.N, d.Ti, d.Hi, d.Wi, d.Cin, d.Cout)))
+            elif name == 'dt_conv1_7x7s2':
+                launched.append((('conv1', a[10], a[11], a[13]), None))
+            elif name == 'dt_conv1_7x7s2_f32':
+                launched.append((('conv1_f32', a[8]), None))
+        assert len(launched) > (50 if run == 'train' or run[0] == 'r50fpn3d' else 20), (run, len(launched))
         record_property('launches_' + tag, len(launched))
         record_property('plan_keys_v2_' + tag, len({k for k, _ in launched}))
         for key, shape in launched:
             seen.add(key)
             if key not in table and key not in conv1_tested:
                 missing.setdefault(key, (tag, shape))
-        del launched[:]
-    try:
-        for wl, modes in (('r50fpn2d', ('bf16x3', 'bf16x3h', 'bf16', 'tf32', 'tf32x3')),
-                          ('r18tube', ('bf16x3', 'bf16x3h', 'bf16', 'tf32', 'tf32x3')), ('r50fpn3d', ('tf32',))):
-            cfg = bench.bench_cfg(800, 1333, wl)
-            blobs, spec = P.random_blobs(cfg)
-            frames = torch.from_numpy(bench.synth_frames(1, bench.frames_per_clip(cfg), 800, 1333, 7)).cuda()
-            for mode in modes:
-                try:
-                    eng = DetectionEngine(cfg, blobs, spec, dtype=mode)
-                except NotImplementedError:
-                    assert mode not in ('bf16', 'bf16x3'), (wl, mode)
-                    record_property('not_taken_%s_%s' % (wl, mode), True)
-                    continue
-                eng.detect(frames)
-                torch.cuda.synchronize()
-                assert len(launched) > 20, (wl, mode, len(launched))
-                check('%s_%s' % (wl, mode))
-                del eng
-        cfg = bench.bench_cfg(800, 1333, 'r50fpn3d')
-        cfg.TRAIN.BATCH_SIZE_PER_IM = 512; cfg.TRAIN.RPN_PRE_NMS_TOP_N = 2000
-        blobs, spec = P.random_blobs(cfg)
-        tr = KeypointRcnnTrainer(cfg, blobs, spec)
-        frames = torch.from_numpy(bench.synth_frames(2, 3, 800, 1333, 100)).cuda()
-        tr.step(frames, pack_gt(bench.synth_gt(2, 800, 1333, 7)))
-        torch.cuda.synchronize()
-        assert len(launched) > 50
-        check('train_forward')
-    finally:
-        from test_gpu_engine import _cfg
-        _cfg()
     record_property('plan_keys_v2_seen', len(seen))
     assert calls['py'] == calls['c'], calls
     assert not missing, missing

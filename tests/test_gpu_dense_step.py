@@ -1,6 +1,6 @@
 """GPU: every launch key of the dense ops on the benchmarked steps (dt_roi_align, dt_roi_align_bwd, dt_maxpool2d, dt_prep_clip,
 dt_keypoint_decode, dt_spatial_mean, dt_fold_tube_heads, dt_scale_rois), launched at the step's shapes on random data and
-compared with the fp64 references of tests/test_dense_reference.py, plus a spy test that proves the table lists every key
+compared with the fp64 references of tests/test_dense_reference.py, plus a coverage test that proves the table lists every key
 that DetectionEngine.detect (r50fpn3d, r50fpn2d, r18tube, every dtype the engine takes) and KeypointRcnnTrainer.step launch.
 
 Tolerances are derived next to each assert (u = 2^-24).  Nothing is tuned to pass."""
@@ -59,64 +59,27 @@ def launch_key(name, a):
     return None
 
 
-def test_step_dense_ops_are_all_in_the_table(monkeypatch, record_property):
+def test_step_dense_ops_are_all_in_the_table(record_property):
     """One 800 x 1333 clip of each bench workload through DetectionEngine.detect in bf16, bf16x3, bf16x3h and tf32x3 (the
     last two where the engine takes them), and one KeypointRcnnTrainer.step at the bench training config: every launch of
     the dense entry points has a key in TABLE, each of which has a value test below."""
-    import bench
-    from detectandtrack_b200 import _lib as L
-    from detectandtrack_b200.modeling import params as Pm
-    from detectandtrack_b200.modeling.engine import DetectionEngine
-    from detectandtrack_b200.modeling.trainer import KeypointRcnnTrainer, pack_gt
-    launched = []
-    orig_call = L.call
-
-    def spy(name, *a):
-        k = launch_key(name, a)
-        if k is not None:
-            launched.append((name, k))
-        return orig_call(name, *a)
-    monkeypatch.setattr(L, 'call', spy)
+    import step_launches as sl
     missing, seen = {}, set()
-    try:
-        for wl in ('r50fpn3d', 'r50fpn2d', 'r18tube'):
-            cfg = bench.bench_cfg(800, 1333, wl)
-            blobs, spec = Pm.random_blobs(cfg)
-            frames = torch.from_numpy(bench.synth_frames(1, bench.frames_per_clip(cfg), 800, 1333, 7)).cuda()
-            for mode in ('bf16', 'bf16x3', 'bf16x3h', 'tf32x3'):
-                del launched[:]
-                try:
-                    eng = DetectionEngine(cfg, blobs, spec, dtype=mode)
-                except NotImplementedError:
-                    assert mode not in ('bf16', 'bf16x3'), (wl, mode)
-                    record_property('not_taken_%s_%s' % (wl, mode), True)
-                    continue
-                eng.detect(frames)
-                torch.cuda.synchronize()
-                record_property('launches_%s_%s' % (wl, mode), len(launched))
-                assert any(n == 'dt_roi_align' for n, _ in launched) and any(n == 'dt_keypoint_decode' for n, _ in launched)
-                for name, k in launched:
-                    seen.add((name, k))
-                    if k not in TABLE[name]:
-                        missing.setdefault((name, k), (wl, mode))
-                del eng
-        cfg = bench.bench_cfg(800, 1333, 'r50fpn3d')
-        cfg.TRAIN.BATCH_SIZE_PER_IM = 512; cfg.TRAIN.RPN_PRE_NMS_TOP_N = 2000
-        blobs, spec = Pm.random_blobs(cfg)
-        tr = KeypointRcnnTrainer(cfg, blobs, spec)
-        frames = torch.from_numpy(bench.synth_frames(2, 3, 800, 1333, 5)).cuda()
-        del launched[:]
-        tr.step(frames, pack_gt(bench.synth_gt(2, 800, 1333, 11)), seed=9)
-        torch.cuda.synchronize()
-        record_property('launches_train', len(launched))
-        assert any(n == 'dt_roi_align_bwd' for n, _ in launched)
+    for run in [(wl, m) for wl in sl.WORKLOADS for m in ('bf16', 'bf16x3', 'bf16x3h', 'tf32x3')] + ['train']:
+        rec = sl.record(run)
+        tag = run if run == 'train' else '%s_%s' % run
+        if not rec.taken:
+            assert run[1] not in ('bf16', 'bf16x3'), run
+            record_property('not_taken_' + tag, True)
+            continue
+        launched = [(name, k) for name, a, _ in rec.calls if (k := launch_key(name, a)) is not None]
+        record_property('launches_' + tag, len(launched))
+        names = {n for n, _ in launched}
+        assert {'dt_roi_align_bwd'} <= names if run == 'train' else {'dt_roi_align', 'dt_keypoint_decode'} <= names
         for name, k in launched:
             seen.add((name, k))
             if k not in TABLE[name]:
-                missing.setdefault((name, k), ('train', 'bf16'))
-    finally:
-        from test_gpu_engine import _cfg
-        _cfg()
+                missing.setdefault((name, k), run)
     record_property('keys_seen', len(seen))
     assert not missing, missing
 

@@ -242,35 +242,15 @@ def test_captured_step_teacher_forced(plan_flip):
         reset_cfg()
 
 
-def test_default_step_launches_no_new_kernel(monkeypatch):
+def test_default_step_launches_no_new_kernel():
     """Both options off: the box stage of a detect call makes exactly the parent's library calls."""
-    sys.path.insert(0, ROOT)
-    import bench
-    from detectandtrack_b200 import _lib as L
-    from detectandtrack_b200.core.config import reset_cfg
-    from detectandtrack_b200.modeling import params as Pm
-    from detectandtrack_b200.modeling.engine import DetectionEngine
-    try:
-        for wl in ('r50fpn3d', 'r18tube'):
-            cfg = bench.bench_cfg(800, 1333, wl)
-            blobs, spec = Pm.random_blobs(cfg)
-            eng = DetectionEngine(cfg, blobs, spec, dtype='bf16x3')
-            names = []
-            real = L.call
-
-            def spy(name, *a):
-                names.append(name)
-                return real(name, *a)
-            monkeypatch.setattr(L, 'call', spy)
-            eng.detect(torch.from_numpy(bench.synth_frames(1, bench.frames_per_clip(cfg), 800, 1333, 7)).cuda())
-            monkeypatch.setattr(L, 'call', real)
-            assert 'dt_soft_nms_batched' not in names and 'dt_box_vote' not in names
-            i = names.index('dt_box_decode')
-            tail = [n for n in names[i + 1:] if n in ('dt_nms_batched', 'dt_limit_detections', 'dt_soft_nms_batched', 'dt_box_vote')]
-            assert tail[:2] == ['dt_nms_batched', 'dt_limit_detections'], tail
-            del eng
-    finally:
-        reset_cfg()
+    import step_launches as sl
+    for wl in ('r50fpn3d', 'r18tube'):
+        names = [name for name, _, _ in sl.record((wl, 'bf16x3')).calls]
+        assert 'dt_soft_nms_batched' not in names and 'dt_box_vote' not in names
+        i = names.index('dt_box_decode')
+        tail = [n for n in names[i + 1:] if n in ('dt_nms_batched', 'dt_limit_detections', 'dt_soft_nms_batched', 'dt_box_vote')]
+        assert tail[:2] == ['dt_nms_batched', 'dt_limit_detections'], tail
 
 
 def test_small_clip_soft_linear_vote_meets_parity_rule(monkeypatch):

@@ -234,70 +234,26 @@ def test_step_launches_only_table_plans_and_keeps_padding_zero():
     TrainConv.backward has a plan key of a TRAIN_STEP row, and after the update the padding filter rows / biases of the
     padded output convs and the dead sub-pixel taps are exactly zero in every copy of the weights (export_blobs relies on
     it)."""
-    import os
-    import sys
-    import torch
-    from detectandtrack_b200.modeling import params as P, trainer as tr_mod
-    from detectandtrack_b200.modeling.trainer import KeypointRcnnTrainer, TrainConv, pack_gt
-    from detectandtrack_b200.ops import conv as cv, train_ops as to
-    from test_conv_plan import plan
-    from test_train_plan import TRAIN_STEP, dgrad_key, wgrad_plan
-    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    import bench
-    cfg = bench.bench_cfg(800, 1333, 'r50fpn3d')
-    cfg.TRAIN.BATCH_SIZE_PER_IM = 512; cfg.TRAIN.RPN_PRE_NMS_TOP_N = 2000
-    blobs, spec = P.random_blobs(cfg)
-    B, T, H, W = cfg.TRAIN.IMS_PER_BATCH, 3, 800, 1333
-    frames = torch.from_numpy(bench.synth_frames(B, T, H, W, 100)).cuda()
-    tr = KeypointRcnnTrainer(cfg, blobs, spec)
-    gt = pack_gt(bench.synth_gt(B, H, W, 7))
+    import collections
+    import ctypes as C
+    from detectandtrack_b200 import _lib as L
+    import step_launches as sl
+    rec = sl.record('train')
     wkeys = {wgrad_key(row_wplan(r)) for r in W_ROWS}
     dkeys = {dgrad_key(row_dplan(r)) for r in D_ROWS}
-    seen_w, seen_d, state = {}, {}, dict(bwd=0)
-    wg, c3, bw = to.wgrad_nhwc, cv.conv3d, TrainConv.backward
-
-    def spy_wgrad(gz, x, ksize, stride=(1, 1), dW=None, cout=None, cin=None):
-        N, T_, Ho, Wo, _ = gz.shape
-        o = wgrad_plan(N, T_, x.shape[2], x.shape[3], cin or x.shape[-1], cout or gz.shape[-1], ksize, tuple(stride))
-        seen_w[wgrad_key(o)] = seen_w.get(wgrad_key(o), 0) + 1
-        return wg(gz, x, ksize, stride, dW, cout=cout, cin=cin)
-
-    def spy_conv(x, w_packed, ksize, stride=(1, 1, 1), pad=(0, 0, 0), *a, **kw):
-        if state['bwd']:
-            N, T_, Hh, Ww, _ = x.shape
-            o = plan(N, T_, Hh, Ww, kw.get('cin') or x.shape[-1], w_packed.shape[1], ksize, stride, pad, res_mode=0, out_f32=0, dtype=0, x3=0)
-            seen_d[dgrad_key(o)] = seen_d.get(dgrad_key(o), 0) + 1
-        return c3(x, w_packed, ksize, stride, pad, *a, **kw)
-
-    def spy_backward(self, *a, **kw):
-        state['bwd'] += 1
-        try:
-            return bw(self, *a, **kw)
-        finally:
-            state['bwd'] -= 1
-    to.wgrad_nhwc, cv.conv3d, TrainConv.backward = spy_wgrad, spy_conv, spy_backward
-    try:
-        tr.step(frames, gt)
-        torch.cuda.synchronize()
-    finally:
-        to.wgrad_nhwc, cv.conv3d, TrainConv.backward = wg, c3, bw
+    seen_w, seen_d = collections.Counter(), collections.Counter()
+    for name, a, in_backward in rec.calls:
+        if name == 'dt_wgrad_nhwc':
+            o = L.WgradPlan()
+            assert L.lib().dt_wgrad_nhwc_plan(a[1], a[3], *a[4:17], C.byref(o)) == 0, L.lib().dt_last_error()
+            seen_w[wgrad_key(o)] += 1
+        elif name == 'dt_conv3d' and in_backward:
+            seen_d[dgrad_key(sl.conv_plan(a)[1])] += 1
     print('wgrad launches %d (%d plans), dgrad launches %d (%d plans)' % (sum(seen_w.values()), len(seen_w), sum(seen_d.values()), len(seen_d)))
     assert set(seen_w) <= wkeys, set(seen_w) - wkeys
     assert set(seen_d) <= dkeys, set(seen_d) - dkeys
-    assert sum(seen_w.values()) == len(tr.convs) + 2 * 4          # the two RPN convs run at five levels
+    assert sum(seen_w.values()) == rec.facts['convs'] + 2 * 4          # the two RPN convs run at five levels
     # padding rows / biases and dead sub-pixel taps stay exactly zero in the master, forward and dgrad filters
-    for c, live in ((tr.rpn_out, 5 * tr.A), (tr.cls_bbox, 5 * tr.C_), (tr.kps_lowres, 4 * tr.K)):
-        assert c.cout > live
-        assert bool((c.w[:, live:] == 0).all()) and bool((c.w_fwd[:, live:] == 0).all()) and bool((c.w_dg[:, :, live:] == 0).all())
-        assert bool((c.bias[live:] == 0).all())
-    K, kl = tr.K, tr.kps_lowres
-    dead = torch.ones((9, kl.cout), dtype=torch.bool)
-    for sub in range(4):
-        py, px = sub >> 1, sub & 1
-        for tap in range(9):
-            dy, dx = tap // 3 - 1, tap % 3 - 1
-            if 0 <= py + 1 - 2 * dy <= 3 and 0 <= px + 1 - 2 * dx <= 3:
-                dead[tap, sub * K:(sub + 1) * K] = False
-    dead = dead.cuda()
-    assert bool((kl.w[dead] == 0).all()) and bool((kl.w_fwd[dead] == 0).all())
-    assert bool((kl.w_dg.flip(0).permute(0, 2, 1)[dead] == 0).all())
+    for name, (rows, w_nonzero, b_nonzero) in rec.facts['padding'].items():
+        assert rows > 0 and w_nonzero == 0 and b_nonzero == 0, name
+    assert rec.facts['dead_taps'][0] > 0 and rec.facts['dead_taps'][1] == 0, rec.facts['dead_taps']

@@ -2,7 +2,7 @@
 dt_rpn_loss_grad / dt_frcnn_loss_grad / dt_kps_loss_grad, the joins dt_bwd_pointwise(2) / dt_upsample_add_bwd /
 dt_scatter_stride2 / dt_embed_frame / dt_grad_join_f32, dt_subpixel_grad_fix, dt_bias_grad and dt_sgd_update_multi),
 launched at the step's shapes on seeded data with edge values and compared element by element with the references of
-tests/test_train_reference.py; a spy test that proves the table lists every key KeypointRcnnTrainer.step (as
+tests/test_train_reference.py; a coverage test that proves the table lists every key KeypointRcnnTrainer.step (as
 `bench.py --train` builds it, and through step_clips at two drawn scales, one clip flipped) and RpnTrainer.step
 (`--train-trunk`) launch; and a teacher-forced capture of one bench step that checks every such launch on its own inputs.
 
@@ -114,50 +114,23 @@ def _num_sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def test_step_train_ops_are_all_in_the_table(step_env, monkeypatch, record_property):
+def test_step_train_ops_are_all_in_the_table(record_property):
     """One KeypointRcnnTrainer.step as bench.py --train runs it, one step_clips of an 800 x 1333 clip at scale 800 and a
     mirrored 720 x 1280 clip drawn to 640 (TRAIN.AUGMENT), and one RpnTrainer.step as --train-trunk runs it: every launch of
     these entry points has a key in TABLE (each with a value test below), and the bench step launches what its graph says."""
-    import bench
-    from detectandtrack_b200 import _lib as L
-    from detectandtrack_b200.modeling.trainer import RpnTrainer, pack_gt
-    launched = []
-    orig_call = L.call
-
-    def spy(name, *a):
-        k = launch_key(name, a)
-        if k is not None:
-            launched.append((name, k))
-        return orig_call(name, *a)
-    monkeypatch.setattr(L, 'call', spy)
+    import step_launches as sl
     missing, seen = {}, set()
-
-    def collect(tag):
+    for tag in ('train', 'augment', 'trunk'):
+        launched = [(name, k) for name, a, _ in sl.record(tag).calls if (k := launch_key(name, a)) is not None]
+        if tag == 'train':
+            counts = collections.Counter(n for n, _ in launched)
+            assert {n: counts[n] for n in STEP_COUNTS} == STEP_COUNTS, dict(counts)
+            assert set(counts) == set(TABLE), set(TABLE) - set(counts)
         for name, k in launched:
             seen.add((name, k))
             if k not in TABLE[name]:
                 missing.setdefault((name, k), tag)
         record_property('launches_%s' % tag, len(launched))
-    tr, cfg = step_env['tr'], step_env['cfg']
-    tr.step(step_env['frames'], step_env['gt'], seed=9)
-    torch.cuda.synchronize()
-    counts = collections.Counter(n for n, _ in launched)
-    assert {n: counts[n] for n in STEP_COUNTS} == STEP_COUNTS, dict(counts)
-    assert set(counts) == set(TABLE), set(TABLE) - set(counts)
-    collect('train')
-    del launched[:]
-    rng = np.random.RandomState(3)
-    clips = [torch.from_numpy(rng.randint(0, 256, (3, h, w, 3)).astype(np.uint8)).cuda() for h, w in ((800, 1333), (720, 1280))]
-    gt = pack_gt(bench.synth_gt(1, 800, 1333, 3) + bench.synth_gt(1, 720, 1280, 4))
-    tr.step_clips(clips, gt, [800, 640], [0, 1], seed=5)
-    torch.cuda.synchronize()
-    collect('augment')
-    del launched[:]
-    rt = RpnTrainer(cfg, step_env['blobs'], step_env['spec'])
-    rt.step(step_env['frames'], rt.synthetic_targets(2, 800, 1333, seed=0))
-    torch.cuda.synchronize()
-    collect('trunk')
-    del rt
     record_property('keys_seen', len(seen))
     for s in sorted(seen, key=str):
         print('  ', s)

@@ -262,35 +262,15 @@ def test_wino_head_vs_direct_head():
     assert (cv.join_split(yw) - cv.join_split(yd)).abs().max().item() <= 1e-3 * cv.join_split(yd).abs().max().item()
 
 
-def _wino_calls(monkeypatch, wl, mode):
-    import bench
-    from detectandtrack_b200 import _lib as L
-    from detectandtrack_b200.modeling import params as P
-    from detectandtrack_b200.modeling.engine import DetectionEngine
-    names = []
-    orig = L.call
-
-    def spy(name, *a):
-        if name.startswith('dt_wino') or (name == 'dt_conv3d' and a[0]._obj.Hi == S and a[0]._obj.kH == 3):
-            names.append(name)
-        return orig(name, *a)
-    monkeypatch.setattr(L, 'call', spy)
-    cfg = bench.bench_cfg(800, 1333, wl)
-    blobs, spec = P.random_blobs(cfg)
-    frames = torch.from_numpy(bench.synth_frames(1, bench.frames_per_clip(cfg), 800, 1333, 7)).cuda()
-    eng = DetectionEngine(cfg, blobs, spec, dtype=mode)
-    eng.detect(frames)
-    torch.cuda.synchronize()
-    monkeypatch.setattr(L, 'call', orig)
-    return eng, names
-
-
 @pytest.mark.parametrize('wl,mode,taken', [('r50fpn3d', 'bf16x3', True), ('r50fpn3d', 'bf16x3h', True),
                                            ('r50fpn3d', 'tf32x3', False), ('r18tube', 'bf16x3', False)])
-def test_engine_takes_the_winograd_path(monkeypatch, wl, mode, taken):
-    eng, names = _wino_calls(monkeypatch, wl, mode)
-    n = len(eng.kps_convs)
-    assert eng.wino_kps == taken
+def test_engine_takes_the_winograd_path(wl, mode, taken):
+    import step_launches as sl
+    rec = sl.record((wl, mode))
+    names = [name for name, a, _ in rec.calls
+             if name.startswith('dt_wino') or (name == 'dt_conv3d' and a[0]._obj.Hi == S and a[0]._obj.kH == 3)]
+    n = rec.facts['kps_convs']
+    assert rec.facts['wino_kps'] == taken
     if taken:
         assert n == 8
         # then the sub-pixel deconv, the one direct 3x3 conv left on the 14 x 14 maps
